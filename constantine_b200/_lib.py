@@ -126,6 +126,10 @@ def load():
     lib.ctt_b200_eth_kzg_compute_cells_and_kzg_proofs_batch.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_kzg_last_das_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 4
     lib.ctt_b200_eth_kzg_last_das_timing.restype = None
+    lib.ctt_b200_eth_kzg_recover_cells_and_kzg_proofs.argtypes = [vp, vp, vp, vp, vp, sz]
+    lib.ctt_b200_eth_kzg_recover_cells_and_kzg_proofs.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_kzg_recover_cells_and_kzg_proofs_batch.argtypes = [vp, vp, vp, vp, vp, vp, sz, ctypes.POINTER(sz)]
+    lib.ctt_b200_eth_kzg_recover_cells_and_kzg_proofs_batch.restype = ctypes.c_ubyte
     lib.ctt_threadpool_new.argtypes = [ci]
     lib.ctt_threadpool_new.restype = vp
     lib.ctt_threadpool_shutdown.argtypes = [vp]

@@ -25,6 +25,9 @@
 // context: cells need only the Fr twiddles every context uploads; the FK20 proofs need the polyphase spectrum bank that
 // ctt_b200_eth_kzg_context_load_peerdas builds once from the monomial setup (reference kzg_multiproofs.nim:227-326). The host checks
 // the blobs, copies cells 0-63 (the blob itself) and compresses the proofs; everything else runs on the device (peerdas_kernels.cuh).
+// Recovery (recover_cells_and_kzg_proofs, reference eth_eip7594_peerdas.nim:621-721) is the same split: the host checks the inputs,
+// lays the present cells out over the extended domain and compresses the proofs; the decode, all 128 cells and the FK20 proofs run on
+// the device.
 #define CTT_B200_BUILDING_LIBRARY
 #include "../../include/ctt_b200_msm.h"
 #include "eth_kzg_host.hpp"
@@ -150,6 +153,24 @@ static void prove(const Context* k, uint8_t* proofs, uint8_t* y, const uint8_t* 
 struct DasTiming { float ms_host = 0, ms_fr = 0, ms_msm = 0, ms_ecfft = 0; };
 static DasTiming& last_das_timing() { static thread_local DasTiming t; return t; }
 
+// n x 128 raw proofs -> n x 128 compressed (one batched inversion)
+static void compress_das_proofs(uint8_t* proofs, const std::vector<HP>& raw, size_t n) {
+  std::vector<Fp> xy(2 * raw.size());
+  batch_affine(raw.data(), raw.size(), xy.data());
+  parallel_for(n, [&](size_t j) {
+    for (size_t i = j * DAS_CELLS; i < (j + 1) * DAS_CELLS; i++)
+      compress_g1(proofs + 48 * i, xy[2 * i], xy[2 * i + 1], raw[i].is_inf());
+  });
+}
+
+static void set_das_timing(double ms_host, const DasTimes& times) {
+  DasTiming& t = last_das_timing();
+  t.ms_host = (float)ms_host;
+  t.ms_fr = times.ms_fr;
+  t.ms_msm = times.ms_msm;
+  t.ms_ecfft = times.ms_ecfft;
+}
+
 // cells (n x 128 x 2048 bytes) and, if proofs is not null, proofs (n x 128 x 48 bytes) of n validated blobs
 static void das(const Context* k, uint8_t* cells, uint8_t* proofs, const uint8_t* blobs, size_t n, double ms_checks) {
   DasBank bank;
@@ -159,19 +180,24 @@ static void das(const Context* k, uint8_t* cells, uint8_t* proofs, const uint8_t
   das_device(k->d_tw, proofs ? &bank : nullptr, blobs, n, cells, raw.data(), &times);
   const auto t0 = std::chrono::steady_clock::now();
   for (size_t j = 0; j < n; j++) memcpy(cells + 2 * BYTES_PER_BLOB * j, blobs + BYTES_PER_BLOB * j, BYTES_PER_BLOB);  // cells 0-63 = the blob
-  if (proofs) {
-    std::vector<Fp> xy(2 * raw.size());
-    batch_affine(raw.data(), raw.size(), xy.data());
-    parallel_for(n, [&](size_t j) {
-      for (size_t i = j * DAS_CELLS; i < (j + 1) * DAS_CELLS; i++)
-        compress_g1(proofs + 48 * i, xy[2 * i], xy[2 * i + 1], raw[i].is_inf());
-    });
+  if (proofs) compress_das_proofs(proofs, raw, n);
+  set_das_timing(ms_checks + ms_since(t0), times);
+}
+
+// recover_cells_and_kzg_proofs' input checks in the reference's order (eth_eip7594_peerdas.nim:645-667): the count (64..128), every
+// index < 128 (all of them before the order is looked at), strictly ascending indices, every element of every cell < r.
+static int check_recovery(const uint64_t* idx, const uint8_t* cells, size_t count) {
+  if (count < DAS_CELLS / 2 || count > DAS_CELLS) return InputsLengthsMismatch;
+  for (size_t i = 0; i < count; i++)
+    if (idx[i] >= DAS_CELLS) return InputsLengthsMismatch;
+  for (size_t i = 1; i < count; i++)
+    if (idx[i - 1] >= idx[i]) return CellIndicesNotAscending;
+  for (size_t e = 0; e < count * (DAS_BYTES_PER_CELL / 32); e++) {
+    uint64_t v[4];
+    be32_to_limbs(v, cells + 32 * e);
+    if (geq_order(v)) return ScalarLargerThanCurveOrder;
   }
-  DasTiming& t = last_das_timing();
-  t.ms_host = (float)(ms_checks + ms_since(t0));
-  t.ms_fr = times.ms_fr;
-  t.ms_msm = times.ms_msm;
-  t.ms_ecfft = times.ms_ecfft;
+  return Success;
 }
 
 // all n blobs checked on host threads; the status of the lowest failing index (and that index), or Success
@@ -200,6 +226,7 @@ ctt_b200_eth_kzg_context* ctt_b200_eth_kzg_context_new(const void* srs_lagrange_
   c->roots = brp_roots_of_unity();   // the proofs' evaluation domain (reference ethereum_kzg_srs.nim:389-394), uploaded once
   c->d_roots = b200::kzg::upload_device(c->roots.data(), c->roots.size() * sizeof(Fr));
   const std::vector<Fr> tw = das_twiddles();   // the EIP-7594 NTTs' roots (compute_cells works on every context)
+  if (tw.size() != DAS_TW_LEN) abort();
   c->d_tw = b200::kzg::upload_device(tw.data(), tw.size() * sizeof(Fr));
   return reinterpret_cast<ctt_b200_eth_kzg_context*>(c);
 }
@@ -384,7 +411,60 @@ unsigned char ctt_b200_eth_kzg_compute_cells_and_kzg_proofs_batch(const ctt_b200
   return (unsigned char)Success;
 }
 
-// the last cells / proofs call of the calling thread
+// reference ctt_eth_kzg_recover_cells_and_kzg_proofs (eth_eip7594_peerdas.nim:621-721); needs load_peerdas
+unsigned char ctt_b200_eth_kzg_recover_cells_and_kzg_proofs(const ctt_b200_eth_kzg_context* ctx, unsigned char* recovered_cells,
+                                                            unsigned char* recovered_proofs, const uint64_t* cell_indices,
+                                                            const unsigned char* cells, size_t num_cells) {
+  return ctt_b200_eth_kzg_recover_cells_and_kzg_proofs_batch(ctx, recovered_cells, recovered_proofs, cell_indices, cells, &num_cells, 1,
+                                                             nullptr);
+}
+
+// n recoveries in one device pass; blob j's indices and cells follow those of blobs 0..j-1. All blobs are checked first; on failure
+// the status of the lowest failing index, that index in *failed_index, outputs untouched
+unsigned char ctt_b200_eth_kzg_recover_cells_and_kzg_proofs_batch(const ctt_b200_eth_kzg_context* ctx, unsigned char* recovered_cells,
+                                                                  unsigned char* recovered_proofs, const uint64_t* cell_indices,
+                                                                  const unsigned char* cells, const size_t* num_cells, size_t n,
+                                                                  size_t* failed_index) {
+  const Context* k = reinterpret_cast<const Context*>(ctx);
+  if (!k || !k->bank) return (unsigned char)VerificationFailure;
+  if (n == 0) return (unsigned char)Success;
+  if (!recovered_cells || !recovered_proofs || !cell_indices || !cells || !num_cells) return (unsigned char)InputsLengthsMismatch;
+  const auto t0 = std::chrono::steady_clock::now();
+  // offsets of each blob's inputs; a count out of range is that blob's failure and ends the walk (later offsets are unknown)
+  std::vector<size_t> off(n, 0);
+  std::vector<int> status(n, Success);
+  size_t walked = n, acc = 0;
+  for (size_t j = 0; j < n; j++) {
+    if (num_cells[j] < DAS_CELLS / 2 || num_cells[j] > DAS_CELLS) { status[j] = InputsLengthsMismatch; walked = j; break; }
+    off[j] = acc;
+    acc += num_cells[j];
+  }
+  parallel_for(walked, [&](size_t j) { status[j] = check_recovery(cell_indices + off[j], cells + DAS_BYTES_PER_CELL * off[j], num_cells[j]); });
+  for (size_t j = 0; j < n; j++)
+    if (status[j] != Success) { if (failed_index) *failed_index = j; return (unsigned char)status[j]; }
+  // the extended evaluations in brp order (cell c holds elements 64 c .. 64 c + 63), zeros at the missing cells
+  std::vector<uint8_t> ext(n * DAS_CELLS * DAS_BYTES_PER_CELL, 0);
+  std::vector<uint32_t> present(4 * n, 0);
+  parallel_for(n, [&](size_t j) {
+    for (size_t i = 0; i < num_cells[j]; i++) {
+      const uint64_t c = cell_indices[off[j] + i];
+      memcpy(&ext[(j * DAS_CELLS + c) * DAS_BYTES_PER_CELL], cells + (off[j] + i) * DAS_BYTES_PER_CELL, DAS_BYTES_PER_CELL);
+      present[4 * j + c / 32] |= 1u << (c % 32);
+    }
+  });
+  const double ms_checks = ms_since(t0);
+  DasBank bank;
+  b200::bases_view(k->bank, &bank.d_points, &bank.table_stride, &bank.force_c);
+  std::vector<HP> raw(n * DAS_CELLS);
+  DasTimes times;
+  recover_device(k->d_tw, bank, ext.data(), present.data(), n, recovered_cells, raw.data(), &times);
+  const auto t1 = std::chrono::steady_clock::now();
+  compress_das_proofs(recovered_proofs, raw, n);
+  set_das_timing(ms_checks + ms_since(t1), times);
+  return (unsigned char)Success;
+}
+
+// the last cells / proofs / recovery call of the calling thread
 void ctt_b200_eth_kzg_last_das_timing(float* ms_host, float* ms_fr, float* ms_msm, float* ms_ecfft) {
   const DasTiming& t = last_das_timing();
   if (ms_host) *ms_host = t.ms_host;

@@ -170,19 +170,32 @@ inline std::vector<Fr> brp_roots_of_unity() {
 }
 
 // The twiddles of the EIP-7594 NTTs (kzg_device.hpp, DAS_TW_LEN): w^k for k < 8192, w = 7^((r - 1) / 8192) (natural order; w^2 is the
-// generator of the 4096-point domain above), then 1/4096 and 1/128. Montgomery form.
+// generator of the 4096-point domain above), then 1/4096 and 1/128, then the recovery's coset tables (coset shift 5, reference
+// eth_peerdas.nim:200): 5^k / 8192 and 5^-k / 8192 for k < 8192, and 5^64. Montgomery form.
 inline std::vector<Fr> das_twiddles() {
   uint64_t e[4];   // (r - 1) / 8192
   for (int i = 0; i < 4; i++) e[i] = ORDER[i];
   e[0] -= 1;
   for (int i = 0; i < 4; i++) e[i] = (e[i] >> 13) | (i + 1 < 4 ? e[i + 1] << 51 : 0);
   const uint64_t seven[4] = {7, 0, 0, 0}, n[4] = {FIELD_ELEMENTS_PER_BLOB, 0, 0, 0}, cds[4] = {128, 0, 0, 0};
+  const uint64_t five[4] = {5, 0, 0, 0}, ext[4] = {8192, 0, 0, 0};
   const Fr w = fr_pow(fr_to_mont(seven), e);
-  std::vector<Fr> tw(8192 + 2);
+  std::vector<Fr> tw(8192 + 2 + 2 * 8192 + 1);
   tw[0] = Fr::one();
   for (size_t k = 1; k < 8192; k++) tw[k] = tw[k - 1] * w;
   tw[8192] = fr_to_mont(n).inv();
   tw[8193] = fr_to_mont(cds).inv();
+  const Fr s = fr_to_mont(five), s_inv = s.inv();
+  Fr up = fr_to_mont(ext).inv(), down = up;
+  for (size_t k = 0; k < 8192; k++) {
+    tw[8194 + k] = up;
+    tw[8194 + 8192 + k] = down;
+    up = up * s;
+    down = down * s_inv;
+  }
+  Fr s64 = Fr::one();
+  for (int k = 0; k < 64; k++) s64 = s64 * s;
+  tw[8194 + 2 * 8192] = s64;
   return tw;
 }
 

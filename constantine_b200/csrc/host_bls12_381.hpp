@@ -11,7 +11,8 @@ namespace bls12_381 {
 
 // reference include/constantine/protocols/ethereum_eip4844_kzg.h:28-39 (cttEthKzg_* status codes)
 enum Status : int { Success = 0, VerificationFailure = 1, InputsLengthsMismatch = 2, ScalarZero = 3, ScalarLargerThanCurveOrder = 4,
-                    EccInvalidEncoding = 5, EccCoordinateGreaterThanOrEqualModulus = 6, EccPointNotOnCurve = 7, EccPointNotInSubgroup = 8 };
+                    EccInvalidEncoding = 5, EccCoordinateGreaterThanOrEqualModulus = 6, EccPointNotOnCurve = 7, EccPointNotInSubgroup = 8,
+                    CellIndicesNotAscending = 9 };
 
 using Fp = host::HFp<Bls12381Fp>;
 

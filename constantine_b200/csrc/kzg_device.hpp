@@ -40,8 +40,11 @@ void prove_device(const void* d_points, size_t table_stride, int force_c, const 
 
 // ---- EIP-7594 cells and FK20 proofs (peerdas_kernels.cuh) --------------------------------------------------------------------
 // d_tw: DAS_TW_LEN Fr Montgomery residues, w^k for k < 8192 (w the 8192-th root of unity of the domain, natural order), then 1/4096
-// and 1/128.
-constexpr size_t DAS_TW_LEN = 8192 + 2;
+// and 1/128 (offsets 8192 and 8193), then the recovery's coset tables: 5^k / 8192 and 5^-k / 8192 for k < 8192, and 5^64.
+constexpr size_t DAS_TW_SHIFT = 8192 + 2;               // 5^k / 8192
+constexpr size_t DAS_TW_UNSHIFT = DAS_TW_SHIFT + 8192;  // 5^-k / 8192
+constexpr size_t DAS_TW_SHIFT64 = DAS_TW_UNSHIFT + 8192;
+constexpr size_t DAS_TW_LEN = DAS_TW_SHIFT64 + 1;
 
 struct DasTimes {
   float ms_fr = 0, ms_msm = 0, ms_ecfft = 0;   // CUDA events: parse + Fr NTT kernels, the bank MSM, the EC FFT kernel
@@ -63,6 +66,13 @@ void das_bank_fft(const void* d_tw, const host::HXyzz<host::HFp<Bls12381Fp>>* in
 // parse, Fr NTTs, bank MSM, EC FFTs, one copy back.
 void das_device(const void* d_tw, const DasBank* bank, const uint8_t* blobs, size_t n, uint8_t* cells,
                 host::HXyzz<host::HFp<Bls12381Fp>>* proofs, DasTimes* times);
+
+// n validated recoveries -> all 128 cells of each (cells: n x 128 x 2048 bytes, canonical big-endian) and its 128 proofs (n x 128
+// raw XYZZ, in cell order). ext: n x 8192 x 32 bytes, the extended evaluations in brp order as cells arrive (big-endian, zeros at the
+// missing cells); present: 4 words per blob, bit c set when cell c is present. One engine lease and stream: parse, the vanishing
+// polynomial, the Reed-Solomon decode and the cells (split 8192-point NTTs), then the FK20 tail of das_device.
+void recover_device(const void* d_tw, const DasBank& bank, const uint8_t* ext, const uint32_t* present, size_t n, uint8_t* cells,
+                    host::HXyzz<host::HFp<Bls12381Fp>>* proofs, DasTimes* times);
 
 }  // namespace kzg
 }  // namespace b200

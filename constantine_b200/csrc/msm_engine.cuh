@@ -172,6 +172,8 @@ struct Engine {
   DeviceBuffer kzg_poly, kzg_args;
   // EIP-7594 cells and proofs (peerdas_kernels.cuh): natural-order coefficients, cells 64-127, the bank MSMs' results, the proofs
   DeviceBuffer das_coefs, das_cells, das_u, das_proofs;
+  // EIP-7594 recovery: the decode's intermediate 8192-point vectors, the present-cell masks and the vanishing polynomial's values
+  DeviceBuffer das_rec, das_z;
   void* h_result = nullptr;   // pinned
   size_t h_result_cap = 0;
   // pinned double buffer through which pageable caller memory is staged (msm_host_on)

@@ -65,6 +65,24 @@ __device__ void das_ntt_smem(uint32_t* s, const uint32_t* __restrict__ tw, bool 
   }
 }
 
+// The 4096 residues in shared memory s -> 4096 x 32 bytes at o (64 cells), canonical big-endian.
+__device__ __forceinline__ void das_store_cells(const uint32_t* s, uint32_t* o) {
+  FrD one_raw = FrD::zero();
+  one_raw.l[0] = 1;
+  for (int i = threadIdx.x; i < KZG_N; i += DAS_NTT_THREADS) {
+    FrD v;
+    load_words_rw(v, s + 8 * i);
+    v = v.mul_u(one_raw);                             // Montgomery -> canonical
+    uint4 lo, hi;                                     // 32 big-endian bytes: word k holds bytes 4k..4k+3, most significant first
+    lo.x = __byte_perm(v.l[7], 0, 0x0123); lo.y = __byte_perm(v.l[6], 0, 0x0123);
+    lo.z = __byte_perm(v.l[5], 0, 0x0123); lo.w = __byte_perm(v.l[4], 0, 0x0123);
+    hi.x = __byte_perm(v.l[3], 0, 0x0123); hi.y = __byte_perm(v.l[2], 0, 0x0123);
+    hi.z = __byte_perm(v.l[1], 0, 0x0123); hi.w = __byte_perm(v.l[0], 0, 0x0123);
+    reinterpret_cast<uint4*>(o)[2 * i] = lo;
+    reinterpret_cast<uint4*>(o)[2 * i + 1] = hi;
+  }
+}
+
 // One block per blob. poly: n x 4096 residues (brp evaluations); coefs: n x 4096 natural-order coefficients (out); cells: n x 4096
 // x 32 bytes, the cells 64..127 of each blob (out).
 __global__ void __launch_bounds__(DAS_NTT_THREADS) k_das_cells(const uint32_t* __restrict__ poly, const uint32_t* __restrict__ tw,
@@ -89,21 +107,7 @@ __global__ void __launch_bounds__(DAS_NTT_THREADS) k_das_cells(const uint32_t* _
   }
   __syncthreads();
   das_ntt_smem<12, true>(s, tw, false);
-  FrD one_raw = FrD::zero();
-  one_raw.l[0] = 1;
-  uint32_t* o = cells + b * (size_t)KZG_N * 8;
-  for (int i = threadIdx.x; i < KZG_N; i += DAS_NTT_THREADS) {
-    FrD v;
-    load_words_rw(v, s + 8 * i);
-    v = v.mul_u(one_raw);                             // Montgomery -> canonical
-    uint4 lo, hi;                                     // 32 big-endian bytes: word k holds bytes 4k..4k+3, most significant first
-    lo.x = __byte_perm(v.l[7], 0, 0x0123); lo.y = __byte_perm(v.l[6], 0, 0x0123);
-    lo.z = __byte_perm(v.l[5], 0, 0x0123); lo.w = __byte_perm(v.l[4], 0, 0x0123);
-    hi.x = __byte_perm(v.l[3], 0, 0x0123); hi.y = __byte_perm(v.l[2], 0, 0x0123);
-    hi.z = __byte_perm(v.l[1], 0, 0x0123); hi.w = __byte_perm(v.l[0], 0, 0x0123);
-    reinterpret_cast<uint4*>(o)[2 * i] = lo;
-    reinterpret_cast<uint4*>(o)[2 * i + 1] = hi;
-  }
+  das_store_cells(s, cells + b * (size_t)KZG_N * 8);
 }
 
 // Two blocks per blob, 32 offsets each. Circulant of offset o (makeCirculantMatrix): c[0] = p[4095 - o], c[128 - j] = p[4095 - o - 64 j]
@@ -139,6 +143,163 @@ __global__ void __launch_bounds__(DAS_NTT_THREADS) k_das_circulants(const uint32
     dst[0] = src[0];
     dst[1] = src[1];
   }
+}
+
+// ---- recovery (recover_cells_and_kzg_proofs) ------------------------------------------------------------------------------------
+// The reference's decode (data_availability_sampling/eth_peerdas.nim:127-225) over the extended domain of 8192 points, with Z(X) =
+// z(X^64), z(y) = prod over missing k of (y - w128^brp7(k)):
+//   D = IFFT(E . FFT(Z)),  coefs = coset-IFFT(coset-FFT(D) / coset-FFT(Z)) (coset shift 5),  cells = FFT(coefs) (all 8192).
+// FFT(Z) at brp index i is z(w128^brp7(i >> 6)) and coset-FFT(Z) is z(5^64 w128^brp7(i >> 6)): 128 values each, one per cell.
+// An 8192-point transform is one radix-2 stage across the two halves plus two independent 4096-point transforms (das_ntt_smem<12>),
+// one block each; the cross stages are fused into the loads of the next kernel:
+//   inverse (brp in, natural out): half 0 -> U, half 1 -> V, a[j] = U[j] + w^-j V[j], a[j + 4096] = U[j] - w^-j V[j];
+//   forward (natural in, brp out): half 0 <- a[j] + a[j + 4096], half 1 <- (a[j] - a[j + 4096]) w^j.
+// tests/peerdas_recovery_exact.py (recovery_model) replays this decomposition over Fr against a transcription of the reference.
+constexpr int REC_N = 2 * KZG_N;         // the extended domain
+constexpr int REC_Z = 2 * DAS_CDS;       // vanishing-polynomial values per blob: 128 on the domain, 128 inverses on the coset
+
+// One block of 256 threads per blob. present: 4 words per blob (bit c: cell c present). zv: per blob, z(w128^brp7(c)) for c < 128
+// (zero at a missing cell), then 1 / z(5^64 w128^brp7(c)): the 128 coset values are inverted together (prefix products, one
+// safegcd inversion, back-substitution).
+__global__ void __launch_bounds__(REC_Z) k_rec_vanishing(const uint32_t* __restrict__ present, const uint32_t* __restrict__ tw,
+                                                         uint32_t* zv) {
+  __shared__ __align__(16) uint32_t zs[DAS_CDS * 8];
+  const size_t b = blockIdx.x;
+  const int t = threadIdx.x, c = t & (DAS_CDS - 1);
+  const bool coset = t >= DAS_CDS;
+  uint32_t pm[4];
+#pragma unroll
+  for (int q = 0; q < 4; q++) pm[q] = present[4 * b + q];
+  FrD x;
+  load_words(x, tw + 8 * (DAS_L * brp7(c)));         // w128^brp7(c) = w8192^(64 brp7(c))
+  if (coset) {
+    FrD s64;
+    load_words(s64, tw + 8 * DAS_TW_SHIFT64);
+    x = x * s64;
+  }
+  FrD z = FrD::one();
+#pragma unroll 1
+  for (int k = 0; k < DAS_CDS; k++) {
+    if ((pm[k >> 5] >> (k & 31)) & 1u) continue;
+    FrD r;
+    load_words(r, tw + 8 * (DAS_L * brp7(k)));
+    z = z * (x - r);
+  }
+  uint32_t* out = zv + b * REC_Z * 8;
+  store_words(coset ? zs + 8 * c : out + 8 * c, z);
+  __syncthreads();
+  if (t != DAS_CDS) return;
+  FrD acc = FrD::one();                               // out[128 + k] <- prefix product of zs[0..k-1]
+#pragma unroll 1
+  for (int k = 0; k < DAS_CDS; k++) {
+    FrD v;
+    load_words_rw(v, zs + 8 * k);
+    store_words(out + 8 * (DAS_CDS + k), acc);
+    acc = acc * v;
+  }
+  FrD inv = fe_inverse(acc);
+#pragma unroll 1
+  for (int k = DAS_CDS - 1; k >= 0; k--) {
+    FrD v, pre;
+    load_words_rw(v, zs + 8 * k);
+    load_words_rw(pre, out + 8 * (DAS_CDS + k));
+    store_words(out + 8 * (DAS_CDS + k), inv * pre);
+    inv = inv * v;
+  }
+}
+
+// The cross stage of an inverse 8192-point transform from its halves U, V (natural order, at uv and uv + 4096 residues), scaled:
+// a0 = (U[j] + w^-j V[j]) sc[j], a1 = (U[j] - w^-j V[j]) sc[j + 4096], sc the table at tw offset sc_off.
+__device__ __forceinline__ void rec_join(const uint32_t* uv, const uint32_t* __restrict__ tw, size_t sc_off, int j, FrD& a0, FrD& a1) {
+  FrD u, v, wi, s0, s1;
+  load_words_rw(u, uv + 8 * j);
+  load_words_rw(v, uv + 8 * (KZG_N + j));
+  load_words(wi, tw + 8 * ((REC_N - j) & (REC_N - 1)));
+  load_words(s0, tw + 8 * (sc_off + j));
+  load_words(s1, tw + 8 * (sc_off + KZG_N + j));
+  const FrD x = v * wi;
+  a0 = (u + x) * s0;
+  a1 = (u - x) * s1;
+}
+
+// The first stage of a forward 8192-point DIF transform: half 0 takes a0 + a1, half 1 takes (a0 - a1) w^j.
+__device__ __forceinline__ FrD rec_split(const FrD& a0, const FrD& a1, const uint32_t* __restrict__ tw, int h, int j) {
+  if (!h) return a0 + a1;
+  FrD w;
+  load_words(w, tw + 8 * j);
+  return (a0 - a1) * w;
+}
+
+// Two blocks per blob, block h owns brp indices h * 4096 .. + 4095. ev: n x 8192 residues, E (brp, zeros at the missing cells),
+// overwritten in place with U (h = 0) and V (h = 1) of IFFT(E . FFT(Z)): E times z on the domain, inverse NTT of 4096 (unscaled:
+// the 1/8192 is in the next kernel's table).
+__global__ void __launch_bounds__(DAS_NTT_THREADS) k_rec_ifft(uint32_t* ev, const uint32_t* zv, const uint32_t* __restrict__ tw) {
+  extern __shared__ __align__(16) uint32_t s[];
+  const size_t b = blockIdx.x >> 1;
+  const int h = blockIdx.x & 1;
+  uint32_t* p = ev + (b * REC_N + (size_t)h * KZG_N) * 8;
+  const uint32_t* zc = zv + b * REC_Z * 8;
+  for (int i = threadIdx.x; i < KZG_N; i += DAS_NTT_THREADS) {
+    FrD v, z;
+    load_words_rw(v, p + 8 * i);
+    load_words_rw(z, zc + 8 * ((h * KZG_N + i) / DAS_L));
+    store_words(s + 8 * i, v * z);
+  }
+  __syncthreads();
+  das_ntt_smem<12, false>(s, tw, true);
+  for (int i = threadIdx.x; i < KZG_N * 2; i += DAS_NTT_THREADS)
+    reinterpret_cast<uint4*>(p)[i] = reinterpret_cast<const uint4*>(s)[i];
+}
+
+// Two blocks per blob. uv: k_rec_ifft's output; out: n x 8192 residues, the halves U', V' of the coset IFFT's inverse transform.
+// D = the joined halves (with 1/8192 and the coset shift 5^k from the table), forward NTT (brp out), divided by Z on the coset
+// (zv's inverses, constant over a cell), inverse NTT of 4096.
+__global__ void __launch_bounds__(DAS_NTT_THREADS) k_rec_coset_divide(const uint32_t* uv, const uint32_t* zv, const uint32_t* __restrict__ tw,
+                                                                      uint32_t* out) {
+  extern __shared__ __align__(16) uint32_t s[];
+  const size_t b = blockIdx.x >> 1;
+  const int h = blockIdx.x & 1;
+  const uint32_t* in = uv + b * REC_N * 8;
+  for (int j = threadIdx.x; j < KZG_N; j += DAS_NTT_THREADS) {
+    FrD a0, a1;
+    rec_join(in, tw, DAS_TW_SHIFT, j, a0, a1);
+    store_words(s + 8 * j, rec_split(a0, a1, tw, h, j));
+  }
+  __syncthreads();
+  das_ntt_smem<12, true>(s, tw, false);
+  const uint32_t* izs = zv + (b * REC_Z + DAS_CDS) * 8;
+  for (int i = threadIdx.x; i < KZG_N; i += DAS_NTT_THREADS) {
+    FrD v, zi;
+    load_words_rw(v, s + 8 * i);
+    load_words_rw(zi, izs + 8 * ((h * KZG_N + i) / DAS_L));
+    store_words(s + 8 * i, v * zi);
+  }
+  __syncthreads();
+  das_ntt_smem<12, false>(s, tw, true);
+  uint32_t* o = out + (b * REC_N + (size_t)h * KZG_N) * 8;
+  for (int i = threadIdx.x; i < KZG_N * 2; i += DAS_NTT_THREADS)
+    reinterpret_cast<uint4*>(o)[i] = reinterpret_cast<const uint4*>(s)[i];
+}
+
+// Two blocks per blob. uv: k_rec_coset_divide's output. The joined halves times 5^-k / 8192 are the 8192 recovered coefficients;
+// block 0 writes coefficients 0..4095 to coefs (n x 4096, the FK20 input). Forward 8192-point NTT (brp out): block h serialises
+// cells 64 h .. 64 h + 63 into cells (n x 8192 x 32 bytes).
+__global__ void __launch_bounds__(DAS_NTT_THREADS) k_rec_cells(const uint32_t* uv, const uint32_t* __restrict__ tw, uint32_t* coefs,
+                                                               uint32_t* cells) {
+  extern __shared__ __align__(16) uint32_t s[];
+  const size_t b = blockIdx.x >> 1;
+  const int h = blockIdx.x & 1;
+  const uint32_t* in = uv + b * REC_N * 8;
+  uint32_t* c = coefs + b * (size_t)KZG_N * 8;
+  for (int j = threadIdx.x; j < KZG_N; j += DAS_NTT_THREADS) {
+    FrD a0, a1;
+    rec_join(in, tw, DAS_TW_UNSHIFT, j, a0, a1);
+    if (!h) store_words(c + 8 * j, a0);
+    store_words(s + 8 * j, rec_split(a0, a1, tw, h, j));
+  }
+  __syncthreads();
+  das_ntt_smem<12, true>(s, tw, false);
+  das_store_cells(s, cells + (b * REC_N + (size_t)h * KZG_N) * 8);
 }
 
 using G1T = Bls12381G1::T;
@@ -245,22 +406,63 @@ void das_bank_fft(const void* d_tw, const host::HXyzz<host::HFp<Bls12381Fp>>* in
   B200_CUDA_CHECK(cudaStreamSynchronize(s));
 }
 
+// the kernels above that take DAS_NTT_SMEM of dynamic shared memory opt in to it once per device
+static void das_smem_opt_in(int device) {
+  static thread_local bool done[MAX_DEVICES] = {};
+  if (done[device]) return;
+  for (const void* f : {(const void*)k_das_cells, (const void*)k_das_circulants, (const void*)k_rec_ifft, (const void*)k_rec_coset_divide,
+                        (const void*)k_rec_cells})
+    B200_CUDA_CHECK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, DAS_NTT_SMEM));
+  done[device] = true;
+}
+
+constexpr size_t DAS_XYZZ_BYTES = 4 * G1T::WORDS * 4;
+
+// The FK20 proofs of n blobs whose coefficients 0..4095 are in E.das_coefs, queued on E's stream: k_das_circulants (then ev[8]), the
+// bank MSM (then ev[11]), k_ec_fft128 (then ev[12]). The n x 128 raw XYZZ proofs are left in E.das_proofs.
+static void das_fk20(Engine& E, const uint32_t* tw, const DasBank& bank, size_t n) {
+  using C = Bls12381G1;
+  cudaStream_t s = E.compute();
+  const size_t nmsm = n * DAS_CDS;
+  E.d_scalars.ensure(nmsm * DAS_L * 32 + 16);
+  k_das_circulants<<<(unsigned)(2 * n), DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((const uint32_t*)E.das_coefs.ptr, tw, (uint32_t*)E.d_scalars.ptr);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
+  E.das_u.ensure(nmsm * DAS_XYZZ_BYTES);
+  E.das_proofs.ensure(nmsm * DAS_XYZZ_BYTES);
+  E.stats.ms_h2d = 0;
+  msm_device<C>(E, E.d_scalars.ptr, bank.d_points, DAS_L, /*fr_mont=*/true, bank.force_c, 0, -1, nullptr, bank.table_stride, nmsm,
+                /*point_sets=*/DAS_CDS, (host::HXyzz<typename C::H>*)E.das_u.ptr, nullptr, nullptr, nullptr, /*batch_out_device=*/true);
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[11], s));
+  k_ec_fft128<true><<<(unsigned)n, DAS_EC_THREADS, 0, s>>>((const uint32_t*)E.das_u.ptr, tw, (uint32_t*)E.das_proofs.ptr);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[12], s));
+}
+
+// After the stream has synchronised: the MSM's phase times, and the call's device phases (ev[7] marks the start of the Fr kernels).
+static void das_collect_times(Engine& E, bool proofs, DasTimes* times) {
+  if (proofs) {
+    collect_msm_times(E);
+    thread_stats() = E.stats;
+  }
+  if (times) {
+    *times = DasTimes();
+    cudaEventElapsedTime(&times->ms_fr, E.ev[7], E.ev[8]);
+    if (proofs) {
+      cudaEventElapsedTime(&times->ms_msm, E.ev[8], E.ev[11]);
+      cudaEventElapsedTime(&times->ms_ecfft, E.ev[11], E.ev[12]);
+    }
+  }
+}
+
 void das_device(const void* d_tw, const DasBank* bank, const uint8_t* blobs, size_t n, uint8_t* cells,
                 host::HXyzz<host::HFp<Bls12381Fp>>* proofs, DasTimes* times) {
-  using C = Bls12381G1;
   if (n == 0) return;
   EngineLease lease = acquire_engine();
   Engine& E = *lease.e;
   cudaStream_t s = E.compute();
-  static thread_local bool smem_opt_in[MAX_DEVICES] = {};
-  if (!smem_opt_in[E.device]) {
-    B200_CUDA_CHECK(cudaFuncSetAttribute(k_das_cells, cudaFuncAttributeMaxDynamicSharedMemorySize, DAS_NTT_SMEM));
-    B200_CUDA_CHECK(cudaFuncSetAttribute(k_das_circulants, cudaFuncAttributeMaxDynamicSharedMemorySize, DAS_NTT_SMEM));
-    smem_opt_in[E.device] = true;
-  }
+  das_smem_opt_in(E.device);
   const size_t elems = n * (size_t)KZG_N, bytes = elems * 32;
-  const size_t nmsm = n * DAS_CDS;
-  constexpr size_t XYZZ_BYTES = 4 * G1T::WORDS * 4;
   E.kzg_poly.ensure(bytes);
   E.das_coefs.ensure(bytes);
   E.das_cells.ensure(bytes);
@@ -270,24 +472,12 @@ void das_device(const void* d_tw, const DasBank* bank, const uint8_t* blobs, siz
   k_kzg_parse<<<(unsigned)((elems + 255) / 256), 256, 0, s>>>((uint32_t*)E.kzg_poly.ptr, elems);
   k_das_cells<<<(unsigned)n, DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((const uint32_t*)E.kzg_poly.ptr, tw, (uint32_t*)E.das_coefs.ptr,
                                                                   (uint32_t*)E.das_cells.ptr);
-  if (bank) {
-    E.d_scalars.ensure(nmsm * DAS_L * 32 + 16);
-    k_das_circulants<<<(unsigned)(2 * n), DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((const uint32_t*)E.das_coefs.ptr, tw, (uint32_t*)E.d_scalars.ptr);
-  }
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
-  if (bank) {
-    E.das_u.ensure(nmsm * XYZZ_BYTES);
-    E.das_proofs.ensure(nmsm * XYZZ_BYTES);
-    E.stats.ms_h2d = 0;
-    msm_device<C>(E, E.d_scalars.ptr, bank->d_points, DAS_L, /*fr_mont=*/true, bank->force_c, 0, -1, nullptr, bank->table_stride, nmsm,
-                  /*point_sets=*/DAS_CDS, (host::HXyzz<typename C::H>*)E.das_u.ptr, nullptr, nullptr, nullptr, /*batch_out_device=*/true);
-    B200_CUDA_CHECK(cudaEventRecord(E.ev[11], s));
-    k_ec_fft128<true><<<(unsigned)n, DAS_EC_THREADS, 0, s>>>((const uint32_t*)E.das_u.ptr, tw, (uint32_t*)E.das_proofs.ptr);
+  if (bank) das_fk20(E, tw, *bank, n);
+  else {
     B200_CUDA_CHECK(cudaGetLastError());
-    B200_CUDA_CHECK(cudaEventRecord(E.ev[12], s));
+    B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
   }
-  const size_t proof_bytes = bank ? nmsm * XYZZ_BYTES : 0;
+  const size_t proof_bytes = bank ? n * DAS_CDS * DAS_XYZZ_BYTES : 0;
   E.ensure_host(bytes + proof_bytes);
   B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, E.das_cells.ptr, bytes, cudaMemcpyDeviceToHost, s));
   if (bank) B200_CUDA_CHECK(cudaMemcpyAsync((char*)E.h_result + bytes, E.das_proofs.ptr, proof_bytes, cudaMemcpyDeviceToHost, s));
@@ -295,19 +485,46 @@ void das_device(const void* d_tw, const DasBank* bank, const uint8_t* blobs, siz
   // cells 64..127 of blob j: the second half of its 128 x 2048 bytes
   for (size_t j = 0; j < n; j++)
     memcpy(cells + (2 * j + 1) * (size_t)KZG_N * 32, (const char*)E.h_result + j * (size_t)KZG_N * 32, (size_t)KZG_N * 32);
-  if (bank) {
-    memcpy((void*)proofs, (const char*)E.h_result + bytes, proof_bytes);
-    collect_msm_times(E);
-    thread_stats() = E.stats;
-  }
-  if (times) {
-    *times = DasTimes();
-    cudaEventElapsedTime(&times->ms_fr, E.ev[7], E.ev[8]);
-    if (bank) {
-      cudaEventElapsedTime(&times->ms_msm, E.ev[8], E.ev[11]);
-      cudaEventElapsedTime(&times->ms_ecfft, E.ev[11], E.ev[12]);
-    }
-  }
+  if (bank) memcpy((void*)proofs, (const char*)E.h_result + bytes, proof_bytes);
+  das_collect_times(E, bank != nullptr, times);
+}
+
+void recover_device(const void* d_tw, const DasBank& bank, const uint8_t* ext, const uint32_t* present, size_t n, uint8_t* cells,
+                    host::HXyzz<host::HFp<Bls12381Fp>>* proofs, DasTimes* times) {
+  if (n == 0) return;
+  EngineLease lease = acquire_engine();
+  Engine& E = *lease.e;
+  cudaStream_t s = E.compute();
+  das_smem_opt_in(E.device);
+  const size_t elems = n * (size_t)REC_N, bytes = elems * 32, mask_bytes = n * 16;
+  E.kzg_poly.ensure(bytes);
+  E.das_rec.ensure(bytes);
+  E.das_cells.ensure(bytes);
+  E.das_coefs.ensure(bytes / 2);
+  E.das_z.ensure(mask_bytes + n * REC_Z * 32);
+  uint32_t* d_present = (uint32_t*)E.das_z.ptr;
+  uint32_t* d_z = (uint32_t*)((char*)E.das_z.ptr + mask_bytes);     // 16 n bytes in: 32-byte residues stay 16-byte aligned
+  const uint32_t* tw = (const uint32_t*)d_tw;
+  B200_CUDA_CHECK(cudaMemcpyAsync(E.kzg_poly.ptr, ext, bytes, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_present, present, mask_bytes, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[7], s));
+  k_kzg_parse<<<(unsigned)((elems + 255) / 256), 256, 0, s>>>((uint32_t*)E.kzg_poly.ptr, elems);
+  k_rec_vanishing<<<(unsigned)n, REC_Z, 0, s>>>(d_present, tw, d_z);
+  k_rec_ifft<<<(unsigned)(2 * n), DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((uint32_t*)E.kzg_poly.ptr, d_z, tw);
+  k_rec_coset_divide<<<(unsigned)(2 * n), DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((const uint32_t*)E.kzg_poly.ptr, d_z, tw,
+                                                                               (uint32_t*)E.das_rec.ptr);
+  k_rec_cells<<<(unsigned)(2 * n), DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((const uint32_t*)E.das_rec.ptr, tw, (uint32_t*)E.das_coefs.ptr,
+                                                                        (uint32_t*)E.das_cells.ptr);
+  B200_CUDA_CHECK(cudaGetLastError());
+  das_fk20(E, tw, bank, n);
+  const size_t proof_bytes = n * DAS_CDS * DAS_XYZZ_BYTES;
+  E.ensure_host(bytes + proof_bytes);
+  B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, E.das_cells.ptr, bytes, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync((char*)E.h_result + bytes, E.das_proofs.ptr, proof_bytes, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  memcpy(cells, E.h_result, bytes);
+  memcpy((void*)proofs, (const char*)E.h_result + bytes, proof_bytes);
+  das_collect_times(E, true, times);
 }
 
 }  // namespace kzg

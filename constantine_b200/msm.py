@@ -444,9 +444,53 @@ class EthKzgContext:
         c, p = self._split(cells.raw, proofs.raw, n)
         return list(zip(c, p))
 
+    def _recovery_inputs(self, items):
+        """[(cell_indices, cells)] -> (uint64 index array, concatenated cells, size_t count array). A cell that is not 2048 bytes, or
+        unequal numbers of indices and cells, raise ValueError(str); counts and index values are left to the library's checks."""
+        idx, cells, counts = [], [], []
+        for j, (cell_indices, blob_cells) in enumerate(items):
+            cell_indices, blob_cells = [int(i) for i in cell_indices], [bytes(c) for c in blob_cells]
+            if len(cell_indices) != len(blob_cells):
+                raise ValueError(f"blob {j}: {len(cell_indices)} cell indices but {len(blob_cells)} cells")
+            for c in blob_cells:
+                self._check_len("cell", c, self.BYTES_PER_CELL)
+            idx += cell_indices
+            cells += blob_cells
+            counts.append(len(blob_cells))
+        return (ctypes.c_uint64 * max(1, len(idx)))(*idx), _buf(b"".join(cells) or b"\0"), (ctypes.c_size_t * max(1, len(counts)))(*counts)
+
+    def recover_cells_and_kzg_proofs(self, cell_indices, cells) -> tuple:
+        """(128 cells, 128 proofs) of the extended blob from at least 64 of its cells and their ascending indices; needs load_peerdas.
+        A status from the library raises ValueError(status)."""
+        idx, cb, counts = self._recovery_inputs([(cell_indices, cells)])
+        out_cells = ctypes.create_string_buffer(self.CELLS_PER_EXT_BLOB * self.BYTES_PER_CELL)
+        out_proofs = ctypes.create_string_buffer(self.CELLS_PER_EXT_BLOB * 48)
+        rc = _lib.load().ctt_b200_eth_kzg_recover_cells_and_kzg_proofs(self._h, out_cells, out_proofs, idx, cb, counts[0])
+        if rc != 0:
+            raise ValueError(rc)
+        c, p = self._split(out_cells.raw, out_proofs.raw, 1)
+        return c[0], p[0]
+
+    def recover_cells_and_kzg_proofs_batch(self, items) -> list:
+        """[(cells, proofs)] for several [(cell_indices, cells)] in one device pass. A bad input raises ValueError(status, index) and
+        nothing is returned."""
+        items = list(items)
+        n = len(items)
+        idx, cb, counts = self._recovery_inputs(items)
+        out_cells = ctypes.create_string_buffer(max(1, n * self.CELLS_PER_EXT_BLOB * self.BYTES_PER_CELL))
+        out_proofs = ctypes.create_string_buffer(max(1, n * self.CELLS_PER_EXT_BLOB * 48))
+        failed = ctypes.c_size_t(0)
+        rc = _lib.load().ctt_b200_eth_kzg_recover_cells_and_kzg_proofs_batch(self._h, out_cells, out_proofs, idx, cb, counts, n,
+                                                                            ctypes.byref(failed))
+        if rc != 0:
+            raise ValueError(rc, failed.value)
+        c, p = self._split(out_cells.raw, out_proofs.raw, n)
+        return list(zip(c, p))
+
     @staticmethod
     def last_das_timing() -> dict:
-        """Host checks + serialisation, Fr kernels, bank MSM and EC FFT time (ms) of the calling thread's last cells / proofs call."""
+        """Host checks + serialisation, Fr kernels, bank MSM and EC FFT time (ms) of the calling thread's last cells / proofs /
+        recovery call."""
         v = [ctypes.c_float(0) for _ in range(4)]
         _lib.load().ctt_b200_eth_kzg_last_das_timing(*[ctypes.byref(x) for x in v])
         return dict(zip(("ms_host", "ms_fr", "ms_msm", "ms_ecfft"), (x.value for x in v)))

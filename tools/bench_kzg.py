@@ -2,11 +2,13 @@
 """EIP-4844 entries on the resident setup: commitments and blob proofs, n single calls against one batched call, with and without
 the window table, and the split of one proof call (host checks + SHA-256, k_kzg_* kernels, MSM). The PeerDAS leg: the one-time
 load_peerdas, compute_cells_and_kzg_proofs as n single calls against one batched call, and the split of a call (host, Fr kernels,
-bank MSM with its engine phases, EC FFTs). Prints one JSON line.
-python tools/bench_kzg.py [--reps R] [--sizes 1,6,9,32,128] [--das-sizes 1,6,21,72]"""
+bank MSM with its engine phases, EC FFTs). The recovery leg: recover_cells_and_kzg_proofs with 64 seeded random cells missing per
+blob, as n single calls against one batched call, and the same split. Prints one JSON line.
+python tools/bench_kzg.py [--reps R] [--sizes 1,6,9,32,128] [--das-sizes 1,6,21,72] [--rec-sizes 1,6,21,72]"""
 import argparse
 import json
 import os
+import random
 import statistics
 import sys
 import time
@@ -63,11 +65,34 @@ def peerdas(ctx, sizes, reps):
     return r
 
 
+def recovery(ctx, sizes, reps):
+    """Needs load_peerdas (the PeerDAS leg runs first). Each blob keeps 64 of its 128 cells, chosen by a seeded generator."""
+    blobs = random_blobs(max(sizes), 7596)
+    rnd = random.Random(7596)
+    items = []
+    for cells, _ in ctx.compute_cells_and_kzg_proofs_batch(blobs):
+        idx = sorted(rnd.sample(range(128), 64))
+        items.append((idx, [cells[i] for i in idx]))
+    r = {}
+    for n in sizes:
+        its = items[:n]
+        r[f"recover_single_x{n}_ms"] = timed(lambda: [ctx.recover_cells_and_kzg_proofs(i, c) for i, c in its], reps)
+        r[f"recover_batched_n{n}_ms"] = timed(lambda: ctx.recover_cells_and_kzg_proofs_batch(its), reps)
+        splits = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            ctx.recover_cells_and_kzg_proofs_batch(its)
+            splits.append({"wall_ms": (time.perf_counter() - t0) * 1e3, **ctx.last_das_timing()})
+        r[f"split_n{n}_ms"] = {k: round(statistics.median(s[k] for s in splits), 3) for k in splits[0]}
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--sizes", default="1,6,9,32,128")
     ap.add_argument("--das-sizes", default="1,6,21,72")
+    ap.add_argument("--rec-sizes", default="1,6,21,72")
     a = ap.parse_args()
     sizes = [int(s) for s in a.sizes.split(",")]
     srs = np.load(os.path.join(ROOT, "tests", "golden", "kzg_commit_kat.npz"))["srs_lagrange_brp_compressed"].tobytes()
@@ -95,6 +120,7 @@ def main():
         r["blob_proof_split_ms"] = {k: round(statistics.median(s[k] for s in splits), 3) for k in splits[0]}
         out["modes"][mode] = r
     out["peerdas"] = peerdas(ctx, [int(s) for s in a.das_sizes.split(",")], a.reps)
+    out["recovery"] = recovery(ctx, [int(s) for s in a.rec_sizes.split(",")], a.reps)
     ctx.delete()
     print(json.dumps(out), flush=True)
 

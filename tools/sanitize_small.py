@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Small MSMs on every curve, meant to run under compute-sanitizer (memcheck / racecheck):
+"""Small MSMs on every curve and a 2-blob PeerDAS recovery, meant to run under compute-sanitizer (memcheck / racecheck):
    compute-sanitizer --tool racecheck python tools/sanitize_small.py"""
 import os, random, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -21,3 +21,14 @@ for cv in CURVES.values():
         got = pyref.jac_bytes_to_affine(M.multi_scalar_mul_vartime_parallel(tp, cv, cb, pb, n), cv)
         want = pyref.jac_bytes_to_affine(oracle.msm(cv, cb, pb, n), cv)
         print(cv.name, n, "all-equal points" if same else "random", "OK" if got == want else "MISMATCH", flush=True)
+
+# a 2-blob recover_cells_and_kzg_proofs batch (recovery kernels, FK20 tail) against compute_cells_and_kzg_proofs
+import numpy as np
+g = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
+commit, das = np.load(os.path.join(g, "kzg_commit_kat.npz")), np.load(os.path.join(g, "peerdas_kat.npz"))
+ctx = M.EthKzgContext(commit["srs_lagrange_brp_compressed"].tobytes(), compressed=True)
+ctx.load_peerdas(das["srs_monomial_compressed"].tobytes())
+full = ctx.compute_cells_and_kzg_proofs_batch([bytes(commit["blobs"][1]), bytes(commit["blobs"][2])])
+items = [(idx, [cells[i] for i in idx]) for idx, (cells, _) in zip((list(range(0, 128, 2)), sorted(r.sample(range(128), 100))), full)]
+print("recovery 2 blobs", "OK" if ctx.recover_cells_and_kzg_proofs_batch(items) == full else "MISMATCH", flush=True)
+ctx.delete()
