@@ -31,10 +31,13 @@
 #define CTT_B200_BUILDING_LIBRARY
 #include "../../include/ctt_b200_msm.h"
 #include "eth_kzg_host.hpp"
+#include "host_pairing.hpp"
 #include "kzg_device.hpp"
 #include <chrono>
 #include <cstdlib>
+#include <string>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 namespace b200 {
@@ -46,10 +49,12 @@ struct Context {
   void* d_roots = nullptr;        // the same, resident
   void* d_tw = nullptr;           // EIP-7594: the 8192-th roots in natural order, 1/4096, 1/128 (das_twiddles), resident
   ctt_b200_bases* bank = nullptr; // EIP-7594: the FK20 polyphase spectrum bank, 128 positions x 64 offsets (load_peerdas)
+  void* d_mono = nullptr;         // EIP-7594 verification: [tau^j]G1 for j < 64, affine Montgomery, resident (load_peerdas)
+  std::vector<G2Aff> g2;          // the 65 monomial G2 points [tau^j]G2 (load_g2_setup); g2[0] is the generator
 };
 
 using HP = host::HXyzz<Fp>;
-constexpr size_t DAS_CELLS = 128, DAS_BYTES_PER_CELL = 2048, DAS_BANK_OFFSETS = 64;
+constexpr size_t DAS_CELLS = 128, DAS_BYTES_PER_CELL = 2048, DAS_BANK_OFFSETS = 64, DAS_L_G2 = 65;
 
 // Every element < r (zero is a valid evaluation). coefs (if not null) receives the canonical little-endian limbs.
 static int check_blob(const uint8_t* blob, uint64_t* coefs) {
@@ -209,6 +214,39 @@ static int check_blobs(const uint8_t* blobs, size_t n, size_t* failed_index) {
   return Success;
 }
 
+// host time of the last verification (input checks + challenge), its device phases and the pairing check (ctt_b200_eth_kzg_last_verify_timing)
+struct VerifyTiming { float ms_host = 0, ms_decode = 0, ms_fr = 0, ms_msm = 0, ms_pairing = 0; };
+static VerifyTiming& last_verify_timing() { static thread_local VerifyTiming t; return t; }
+
+// The byte-level part of decompress_g1 (flags, x < p) for the device decoder
+static VerifyPoint verify_point(const uint8_t src[48]) {
+  VerifyPoint v;
+  memset(&v, 0, sizeof(v));
+  const uint8_t flags = src[0];
+  if (!(flags & 0x80)) { v.mode = EccInvalidEncoding; return v; }
+  if (flags & 0x40) {
+    bool clean = !(flags & 0x3F);
+    for (int i = 1; i < 48; i++) clean = clean && !src[i];
+    v.mode = clean ? VER_INFINITY : (uint32_t)EccInvalidEncoding;
+    return v;
+  }
+  Fp raw;
+  if (!read_fp(raw, src, true)) { v.mode = EccCoordinateGreaterThanOrEqualModulus; return v; }
+  for (int i = 0; i < 6; i++) { v.x[2 * i] = (uint32_t)raw.l[i]; v.x[2 * i + 1] = (uint32_t)(raw.l[i] >> 32); }
+  v.mode = VER_DECODE;
+  v.sign = (flags & 0x20) ? 1 : 0;
+  return v;
+}
+
+static G1Aff xyzz_affine(const HP& p) {
+  G1Aff a;
+  if (p.is_inf()) { a.x = Fp::zero(); a.y = Fp::zero(); return a; }
+  const Fp di = (p.zz * p.zzz).inv();
+  a.x = p.x * (di * p.zzz);
+  a.y = p.y * (di * p.zz);
+  return a;
+}
+
 }  // namespace kzg
 }  // namespace b200
 
@@ -255,6 +293,7 @@ void ctt_b200_eth_kzg_context_delete(ctt_b200_eth_kzg_context* ctx) {
   if (!k) return;
   ctt_b200_bases_free(k->bases);
   ctt_b200_bases_free(k->bank);
+  b200::kzg::free_device(k->d_mono);
   b200::kzg::free_device(k->d_roots);
   b200::kzg::free_device(k->d_tw);
   delete k;
@@ -376,7 +415,148 @@ int ctt_b200_eth_kzg_context_load_peerdas(ctt_b200_eth_kzg_context* ctx, const u
   if (ctt_b200_bases_precompute_for(bank, DAS_BANK_OFFSETS, 0) < 0) { ctt_b200_bases_free(bank); return VerificationFailure; }
   ctt_b200_bases_free(k->bank);
   k->bank = bank;
+  void* mono = b200::kzg::upload_device(s.data(), 2 * DAS_BANK_OFFSETS * sizeof(Fp));   // [tau^j]G1, j < 64, for the verification
+  b200::kzg::free_device(k->d_mono);
+  k->d_mono = mono;
   return Success;
+}
+
+// One-time: the 65 monomial G2 points of the trusted setup (96-byte compressed, file order), decoded and checked (curve, subgroup).
+// The batch verification uses [tau^64]G2 and [1]G2 = g2[0]. Returns the status of the first bad point (the context is unchanged then).
+int ctt_b200_eth_kzg_context_load_g2_setup(ctt_b200_eth_kzg_context* ctx, const unsigned char* srs_monomial_g2_compressed) {
+  Context* k = reinterpret_cast<Context*>(ctx);
+  if (!k || !srs_monomial_g2_compressed) return VerificationFailure;
+  std::vector<G2Aff> g2(DAS_L_G2);
+  std::vector<int> status(DAS_L_G2);
+  parallel_for(DAS_L_G2, [&](size_t i) { status[i] = check_g2(g2[i], srs_monomial_g2_compressed + 96 * i); });
+  for (int st : status)
+    if (st != Success) return st;
+  k->g2 = g2;
+  return Success;
+}
+
+// reference ctt_eth_kzg_verify_cell_kzg_proof_batch (eth_eip7594_peerdas.nim:509-619); needs load_peerdas and load_g2_setup.
+// Checks in the reference's order, the status of the first failing one: the indices (< 128), the unique commitments (deduplicated on
+// their bytes, first occurrence kept, decoded in that order), every cell element < r, every proof. Success when the pairing check
+// holds, VerificationFailure when it does not.
+unsigned char ctt_b200_eth_kzg_verify_cell_kzg_proof_batch(const ctt_b200_eth_kzg_context* ctx, const unsigned char* commitments,
+                                                           const uint64_t* cell_indices, const unsigned char* cells,
+                                                           const unsigned char* proofs, size_t num_cells,
+                                                           const unsigned char secure_random_bytes[32]) {
+  const Context* k = reinterpret_cast<const Context*>(ctx);
+  if (!k || !k->d_mono || k->g2.size() != DAS_L_G2) return (unsigned char)VerificationFailure;
+  const size_t n = num_cells;
+  if (n == 0) return (unsigned char)Success;
+  if (!commitments || !cell_indices || !cells || !proofs || !secure_random_bytes) return (unsigned char)InputsLengthsMismatch;
+  const auto t0 = std::chrono::steady_clock::now();
+  for (size_t i = 0; i < n; i++)
+    if (cell_indices[i] >= DAS_CELLS) return (unsigned char)InputsLengthsMismatch;
+  // unique commitments on their bytes, in order of first occurrence
+  std::unordered_map<std::string, uint32_t> seen;
+  std::vector<uint64_t> cidx(n);
+  std::vector<size_t> first;
+  for (size_t i = 0; i < n; i++) {
+    auto it = seen.emplace(std::string((const char*)commitments + 48 * i, 48), (uint32_t)first.size());
+    if (it.second) first.push_back(i);
+    cidx[i] = it.first->second;
+  }
+  const size_t U = first.size();
+  std::vector<VerifyPoint> pts(n + U);
+  for (size_t i = 0; i < n; i++) pts[i] = verify_point(proofs + 48 * i);
+  for (size_t u = 0; u < U; u++) pts[n + u] = verify_point(commitments + 48 * first[u]);
+  // counting sorts: the cells of each used column, the cells of each commitment; every cell's column
+  std::vector<uint32_t> col_count(DAS_CELLS, 0), com_count(U, 0);
+  for (size_t i = 0; i < n; i++) { col_count[cell_indices[i]]++; com_count[cidx[i]]++; }
+  std::vector<uint32_t> slot(DAS_CELLS, 0), idx;
+  std::vector<uint32_t> col_id, col_start;
+  for (uint32_t c = 0; c < DAS_CELLS; c++)
+    if (col_count[c]) { col_id.push_back(c); }
+  const size_t used = col_id.size();
+  idx.reserve(used + used + 1 + n + U + 1 + n + n);
+  idx.insert(idx.end(), col_id.begin(), col_id.end());
+  uint32_t acc = 0;
+  for (size_t u = 0; u < used; u++) { idx.push_back(acc); slot[col_id[u]] = acc; acc += col_count[col_id[u]]; }
+  idx.push_back(acc);
+  const size_t o_col_list = idx.size();
+  idx.resize(idx.size() + n);
+  for (size_t i = 0; i < n; i++) idx[o_col_list + slot[cell_indices[i]]++] = (uint32_t)i;
+  std::vector<uint32_t> com_slot(U);
+  acc = 0;
+  for (size_t u = 0; u < U; u++) { idx.push_back(acc); com_slot[u] = acc; acc += com_count[u]; }
+  idx.push_back(acc);
+  const size_t o_com_list = idx.size();
+  idx.resize(idx.size() + n);
+  for (size_t i = 0; i < n; i++) idx[o_com_list + com_slot[cidx[i]]++] = (uint32_t)i;
+  for (size_t i = 0; i < n; i++) idx.push_back((uint32_t)cell_indices[i]);
+  VerifyBatch vb;
+  vb.n = n; vb.U = U; vb.used_cols = used;
+  vb.points = pts.data(); vb.cells = cells; vb.index_words = idx.data();
+
+  double ms_host = ms_since(t0);
+  int cell_status = Success;
+  uint64_t r[4] = {0, 0, 0, 0};
+  auto overlap = [&] {
+    const auto t1 = std::chrono::steady_clock::now();
+    std::vector<int> bad(n, 0);
+    parallel_for((n + 255) / 256, [&](size_t b) {
+      for (size_t i = 256 * b; i < n && i < 256 * (b + 1); i++)
+        for (size_t e = 0; e < DAS_BYTES_PER_CELL / 32; e++) {
+          uint64_t v[4];
+          be32_to_limbs(v, cells + DAS_BYTES_PER_CELL * i + 32 * e);
+          if (geq_order(v)) { bad[i] = 1; break; }
+        }
+    });
+    for (size_t i = 0; i < n; i++)
+      if (bad[i]) { cell_status = ScalarLargerThanCurveOrder; break; }
+    if (cell_status == Success) {
+      reduce_be32(r, secure_random_bytes);                       // getBatchBlindingFactor, else the Fiat-Shamir challenge
+      if ((r[0] | r[1] | r[2] | r[3]) == 0) {
+        std::vector<uint8_t> uniq(48 * U);
+        for (size_t u = 0; u < U; u++) memcpy(&uniq[48 * u], commitments + 48 * first[u], 48);
+        cell_batch_challenge(r, uniq.data(), U, cidx.data(), cell_indices, cells, proofs, n);
+      }
+    }
+    ms_host += ms_since(t1);
+  };
+  auto decide = [&](const uint8_t* st) -> int {
+    for (size_t u = 0; u < U; u++)
+      if (st[n + u]) return st[n + u];
+    if (cell_status != Success) return cell_status;
+    for (size_t i = 0; i < n; i++)
+      if (st[i]) return st[i];
+    return Success;
+  };
+  auto challenge = [&](uint64_t* out) {
+    const Fr rm = fr_to_mont(r);
+    memcpy(out, rm.l, 32);
+  };
+  HP res[2];
+  VerifyTimes times;
+  const int st = verify_device(k->d_tw, k->d_mono, vb, overlap, decide, challenge, res, &times);
+  VerifyTiming& tm = last_verify_timing();
+  tm = VerifyTiming();
+  tm.ms_host = (float)ms_host;
+  tm.ms_decode = times.ms_decode;
+  if (st != Success) return (unsigned char)st;
+  tm.ms_fr = times.ms_fr;
+  tm.ms_msm = times.ms_msm;
+  const auto t2 = std::chrono::steady_clock::now();
+  G2Aff neg_g2 = k->g2[0];
+  neg_g2.y = neg_g2.y.neg();
+  const bool ok = pairing_check(xyzz_affine(res[0]), k->g2[DAS_L_G2 - 1], xyzz_affine(res[1]), neg_g2);
+  tm.ms_pairing = (float)ms_since(t2);
+  return (unsigned char)(ok ? Success : VerificationFailure);
+}
+
+// the last verify_cell_kzg_proof_batch call of the calling thread: host checks + challenge, the device decode, the scalar kernels and
+// the bank MSM (CUDA events), and the host pairing check
+void ctt_b200_eth_kzg_last_verify_timing(float* ms_host, float* ms_decode, float* ms_fr, float* ms_msm, float* ms_pairing) {
+  const VerifyTiming& t = last_verify_timing();
+  if (ms_host) *ms_host = t.ms_host;
+  if (ms_decode) *ms_decode = t.ms_decode;
+  if (ms_fr) *ms_fr = t.ms_fr;
+  if (ms_msm) *ms_msm = t.ms_msm;
+  if (ms_pairing) *ms_pairing = t.ms_pairing;
 }
 
 // reference ctt_eth_kzg_compute_cells (eth_eip7594_peerdas.nim:207-265): the 128 cells of the extended blob

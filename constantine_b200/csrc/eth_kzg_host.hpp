@@ -116,6 +116,19 @@ inline void fr_from_mont(uint64_t canonical[4], const Fr& m) {
   for (int i = 0; i < 4; i++) canonical[i] = v.l[i];
 }
 
+// 32 big-endian bytes reduced mod r (hash_to_bls_field; also the blinding factor taken from caller-supplied random bytes)
+inline void reduce_be32(uint64_t z[4], const uint8_t src[32]) {
+  be32_to_limbs(z, src);
+  while (geq_order(z)) {   // a 256-bit value is below 3r: at most two subtractions
+    unsigned __int128 borrow = 0;
+    for (int i = 0; i < 4; i++) {
+      const unsigned __int128 d = (unsigned __int128)z[i] - ORDER[i] - borrow;
+      z[i] = (uint64_t)d;
+      borrow = (d >> 64) & 1;
+    }
+  }
+}
+
 // ---- Fiat-Shamir challenge of compute_blob_kzg_proof (reference ethereum_eip4844_kzg.nim:126-146, hash_to_bls_field :111-124)
 // SHA-256("FSBLOBVERIFY_V1_" || 8 zero bytes || u64be(4096) || blob || commitment), read big-endian and reduced mod r.
 inline void fiat_shamir_challenge(uint64_t z[4], const uint8_t* blob, const uint8_t commitment[48]) {
@@ -129,15 +142,37 @@ inline void fiat_shamir_challenge(uint64_t z[4], const uint8_t* blob, const uint
   s.update(commitment, 48);
   uint8_t digest[32];
   s.finish(digest);
-  be32_to_limbs(z, digest);
-  while (geq_order(z)) {   // a 256-bit value is below 3r: at most two subtractions
-    unsigned __int128 borrow = 0;
-    for (int i = 0; i < 4; i++) {
-      const unsigned __int128 d = (unsigned __int128)z[i] - ORDER[i] - borrow;
-      z[i] = (uint64_t)d;
-      borrow = (d >> 64) & 1;
-    }
+  reduce_be32(z, digest);
+}
+
+// ---- Fiat-Shamir challenge of verify_cell_kzg_proof_batch (reference eth_eip7594_peerdas.nim:475-507) ---------------------------
+// SHA-256("RCKZGCBATCH__V1_" || u64be(4096) || u64be(64) || u64be(U) || u64be(n) || the U unique commitments || per cell k:
+// u64be(commitment_idx[k]) || u64be(cell_indices[k]) || its 64 elements (32 bytes big-endian each) || proof k), reduced mod r.
+// The cells are hashed as given: canonical big-endian is exactly what the range check of the elements has established.
+inline void put_u64be(Sha256& s, uint64_t v) {
+  uint8_t b[8];
+  for (int i = 0; i < 8; i++) b[i] = (uint8_t)(v >> (56 - 8 * i));
+  s.update(b, 8);
+}
+inline void cell_batch_challenge(uint64_t r[4], const uint8_t* unique_commitments, size_t num_unique, const uint64_t* commitment_idx,
+                                 const uint64_t* cell_indices, const uint8_t* cells, const uint8_t* proofs, size_t n) {
+  static const char DOMAIN[] = "RCKZGCBATCH__V1_";
+  Sha256 s;
+  s.update((const uint8_t*)DOMAIN, 16);
+  put_u64be(s, FIELD_ELEMENTS_PER_BLOB);
+  put_u64be(s, 64);
+  put_u64be(s, num_unique);
+  put_u64be(s, n);
+  s.update(unique_commitments, 48 * num_unique);
+  for (size_t k = 0; k < n; k++) {
+    put_u64be(s, commitment_idx[k]);
+    put_u64be(s, cell_indices[k]);
+    s.update(cells + 2048 * k, 2048);
+    s.update(proofs + 48 * k, 48);
   }
+  uint8_t digest[32];
+  s.finish(digest);
+  reduce_be32(r, digest);
 }
 
 // ---- evaluation domain (reference commitments_setups/ethereum_kzg_srs.nim:389-394) --------------------------------------
@@ -171,7 +206,8 @@ inline std::vector<Fr> brp_roots_of_unity() {
 
 // The twiddles of the EIP-7594 NTTs (kzg_device.hpp, DAS_TW_LEN): w^k for k < 8192, w = 7^((r - 1) / 8192) (natural order; w^2 is the
 // generator of the 4096-point domain above), then 1/4096 and 1/128, then the recovery's coset tables (coset shift 5, reference
-// eth_peerdas.nim:200): 5^k / 8192 and 5^-k / 8192 for k < 8192, and 5^64. Montgomery form.
+// eth_peerdas.nim:200): 5^k / 8192 and 5^-k / 8192 for k < 8192, and 5^64, then 1/64 (the verification's 64-point inverse NTTs).
+// Montgomery form.
 inline std::vector<Fr> das_twiddles() {
   uint64_t e[4];   // (r - 1) / 8192
   for (int i = 0; i < 4; i++) e[i] = ORDER[i];
@@ -180,7 +216,7 @@ inline std::vector<Fr> das_twiddles() {
   const uint64_t seven[4] = {7, 0, 0, 0}, n[4] = {FIELD_ELEMENTS_PER_BLOB, 0, 0, 0}, cds[4] = {128, 0, 0, 0};
   const uint64_t five[4] = {5, 0, 0, 0}, ext[4] = {8192, 0, 0, 0};
   const Fr w = fr_pow(fr_to_mont(seven), e);
-  std::vector<Fr> tw(8192 + 2 + 2 * 8192 + 1);
+  std::vector<Fr> tw(8192 + 2 + 2 * 8192 + 2);
   tw[0] = Fr::one();
   for (size_t k = 1; k < 8192; k++) tw[k] = tw[k - 1] * w;
   tw[8192] = fr_to_mont(n).inv();
@@ -196,6 +232,8 @@ inline std::vector<Fr> das_twiddles() {
   Fr s64 = Fr::one();
   for (int k = 0; k < 64; k++) s64 = s64 * s;
   tw[8194 + 2 * 8192] = s64;
+  const uint64_t cell[4] = {64, 0, 0, 0};
+  tw[8194 + 2 * 8192 + 1] = fr_to_mont(cell).inv();
   return tw;
 }
 

@@ -4,6 +4,7 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <functional>
 #include "host_field.hpp"
 
 struct ctt_b200_bases;
@@ -40,11 +41,13 @@ void prove_device(const void* d_points, size_t table_stride, int force_c, const 
 
 // ---- EIP-7594 cells and FK20 proofs (peerdas_kernels.cuh) --------------------------------------------------------------------
 // d_tw: DAS_TW_LEN Fr Montgomery residues, w^k for k < 8192 (w the 8192-th root of unity of the domain, natural order), then 1/4096
-// and 1/128 (offsets 8192 and 8193), then the recovery's coset tables: 5^k / 8192 and 5^-k / 8192 for k < 8192, and 5^64.
+// and 1/128 (offsets 8192 and 8193), then the recovery's coset tables: 5^k / 8192 and 5^-k / 8192 for k < 8192, and 5^64, then the
+// verification's 1/64.
 constexpr size_t DAS_TW_SHIFT = 8192 + 2;               // 5^k / 8192
 constexpr size_t DAS_TW_UNSHIFT = DAS_TW_SHIFT + 8192;  // 5^-k / 8192
 constexpr size_t DAS_TW_SHIFT64 = DAS_TW_UNSHIFT + 8192;
-constexpr size_t DAS_TW_LEN = DAS_TW_SHIFT64 + 1;
+constexpr size_t DAS_TW_INV64 = DAS_TW_SHIFT64 + 1;
+constexpr size_t DAS_TW_LEN = DAS_TW_INV64 + 1;
 
 struct DasTimes {
   float ms_fr = 0, ms_msm = 0, ms_ecfft = 0;   // CUDA events: parse + Fr NTT kernels, the bank MSM, the EC FFT kernel
@@ -73,6 +76,40 @@ void das_device(const void* d_tw, const DasBank* bank, const uint8_t* blobs, siz
 // polynomial, the Reed-Solomon decode and the cells (split 8192-point NTTs), then the FK20 tail of das_device.
 void recover_device(const void* d_tw, const DasBank& bank, const uint8_t* ext, const uint32_t* present, size_t n, uint8_t* cells,
                     host::HXyzz<host::HFp<Bls12381Fp>>* proofs, DasTimes* times);
+
+// ---- EIP-7594 batch verification (verify_kernels.cuh) ------------------------------------------------------------------------
+// One compressed G1 point after the host's byte-level checks: x canonical (12 little-endian 32-bit words), the sign flag, and what the
+// device has to do with it (decode it, write infinity, or only report the status the host found: 5 or 6).
+constexpr uint32_t VER_DECODE = 0, VER_INFINITY = 1;
+struct VerifyPoint {
+  uint32_t x[12];
+  uint32_t mode;      // VER_DECODE, VER_INFINITY, or a cttEthKzg status
+  uint32_t sign;      // the 0x20 flag: y is the larger root
+  uint32_t pad[2];
+};
+static_assert(sizeof(VerifyPoint) == 64, "VerifyPoint layout");
+
+// The inputs of one verification after the host's checks. points: n proofs then U unique commitments; cells: n x 2048 bytes as given;
+// index_words: used column ids, column starts (used + 1), the cells of each column (n, counting-sorted), commitment starts (U + 1),
+// the cells of each commitment (n), and every cell's column (n).
+struct VerifyBatch {
+  size_t n = 0, U = 0, used_cols = 0;
+  const VerifyPoint* points = nullptr;
+  const uint8_t* cells = nullptr;
+  const uint32_t* index_words = nullptr;
+};
+
+struct VerifyTimes {
+  float ms_decode = 0, ms_fr = 0, ms_msm = 0;   // CUDA events: k_ver_decode; the parse and scalar kernels; the bank MSM
+};
+
+// One engine lease and stream. Uploads and decodes the points, then runs `overlap` on the host (the cell checks and the challenge) while
+// the device works, synchronises and calls `decide` with the per-point statuses; a non-zero result is returned as it is. Otherwise
+// `challenge` writes r (Fr Montgomery, 4 limbs), the scalar kernels and the bank of 2 MSMs run, and out[0] = sum r^k pi_k,
+// out[1] = sum r^k h_k^64 pi_k + sum w_i C_i - [I(tau)]G1 (raw XYZZ). d_mono: the 64 monomial setup points [tau^j]G1, affine.
+int verify_device(const void* d_tw, const void* d_mono, const VerifyBatch& vb, const std::function<void()>& overlap,
+                  const std::function<int(const uint8_t*)>& decide, const std::function<void(uint64_t*)>& challenge,
+                  host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times);
 
 }  // namespace kzg
 }  // namespace b200

@@ -174,6 +174,8 @@ struct Engine {
   DeviceBuffer das_coefs, das_cells, das_u, das_proofs;
   // EIP-7594 recovery: the decode's intermediate 8192-point vectors, the present-cell masks and the vanishing polynomial's values
   DeviceBuffer das_rec, das_z;
+  // EIP-7594 batch verification: the inputs (points, cells, index lists, r), the MSM point set, statuses / powers / column results
+  DeviceBuffer ver_in, ver_pts, ver_aux;
   void* h_result = nullptr;   // pinned
   size_t h_result_cap = 0;
   // pinned double buffer through which pageable caller memory is staged (msm_host_on)

@@ -1,0 +1,273 @@
+// EIP-7594 (PeerDAS) batch verification on the device: verify_cell_kzg_proof_batch (kzg_device.hpp declares the interface;
+// eth_kzg_commit.cu is the host side). Reference eth_eip7594_peerdas.nim:509-619 and kzg_multiproofs.nim:508-736 (kzg_coset_verify_batch):
+//   e(sum_k r^k pi_k, [tau^64]G2) = e(sum_k r^k h_k^64 pi_k + sum_i (sum_{k in row i} r^k) C_i - [sum_k r^k I_k(tau)]G1, G2).
+// Per call, on one engine lease and stream:
+//   1. k_ver_decode: one thread per point (the n proofs, then the U unique commitments): the host has done the byte-level part of the
+//      compressed format (flags, x < p); the kernel takes y = (x^3 + 4)^((p+1)/4), checks it, picks the sign and checks [r]P = O with
+//      the XYZZ formulas (the same double-and-add chain as the host's in_subgroup), and writes the affine point straight into the
+//      MSM point set, plus one status byte per point. The cells are parsed (k_kzg_parse) behind it while the host hashes.
+//   2. after the host has read the statuses and chosen r: k_ver_powers (r^1 .. r^n), k_ver_scalars (row A = r^k; row B = r^k h_k^64 and
+//      the per-commitment sums of r^k), k_ver_columns (one block per used column: sum_k r^k evals_k, the 64-point coset inverse NTT with
+//      shift h_c = w8192^brp7(c)), k_ver_interp (the column results summed and negated into row B);
+//   3. the engine: a bank of 2 MSMs over one shared point set [proofs | unique commitments | [tau^j]G1, j < 64].
+// The pairing check is host code (host_pairing.hpp). tests/peerdas_verify_exact.py computes the same scalars in Python.
+// Included by inst_bls12_381_g1.cu only, next to the engine instantiation it runs.
+#pragma once
+#include "peerdas_kernels.cuh"
+
+namespace b200 {
+namespace kzg {
+
+using FpD = Fp<Bls12381Fp>;
+constexpr int VER_THREADS = 128;
+
+// p's words with a small constant added and shifted right: ((p + add) >> shift), 12 little-endian 32-bit words
+__device__ __forceinline__ void ver_p_words(uint32_t* e, uint32_t add, int shift) {
+  uint64_t carry = add;
+#pragma unroll
+  for (int i = 0; i < 12; i++) { const uint64_t v = (uint64_t)Bls12381Fp::P(i) + carry; e[i] = (uint32_t)v; carry = v >> 32; }
+#pragma unroll
+  for (int i = 0; i < 12; i++) e[i] = (e[i] >> shift) | (i + 1 < 12 ? e[i + 1] << (32 - shift) : 0u);
+}
+
+// in: per point VER_IN_WORDS words (kzg_device.hpp, VerifyPoint); pts: affine Montgomery (x, y), (0, 0) for infinity; status: per point
+__global__ void __launch_bounds__(VER_THREADS) k_ver_decode(const VerifyPoint* __restrict__ in, size_t count, uint32_t* pts, uint8_t* status) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const VerifyPoint v = in[i];
+  uint32_t* o = pts + i * 2 * FpD::WORDS;
+  if (v.mode != VER_DECODE) {                         // infinity (valid) or a status the host has already found
+    store_words(o, FpD::zero());
+    store_words(o + FpD::WORDS, FpD::zero());
+    status[i] = v.mode == VER_INFINITY ? (uint8_t)0 : (uint8_t)v.mode;
+    return;
+  }
+  FpD x, r2, one_raw = FpD::zero();
+#pragma unroll
+  for (int w = 0; w < 12; w++) { x.l[w] = v.x[w]; r2.l[w] = Bls12381Fp::R2(w); }
+  one_raw.l[0] = 1;
+  x = x.mul_u(r2);
+  FpD four = FpD::one().dbl();
+  four = four.dbl();
+  const FpD rhs = x.sqr() * x + four;
+  uint32_t e[12];
+  ver_p_words(e, 1, 2);                               // (p + 1) / 4
+  FpD y = FpD::one();
+#pragma unroll 1
+  for (int b = 380; b >= 0; b--) {
+    y = y.sqr();
+    if ((e[b >> 5] >> (b & 31)) & 1u) y = y * rhs;
+  }
+  if (!(y.sqr() == rhs)) { status[i] = 7; store_words(o, FpD::zero()); store_words(o + FpD::WORDS, FpD::zero()); return; }
+  // sign: y > (p - 1) / 2 as integers
+  const FpD yc = y.mul_u(one_raw);
+  ver_p_words(e, 0, 1);                               // (p - 1) / 2 (p is odd: the shift drops the 1)
+  bool larger = false;
+#pragma unroll 1
+  for (int w = 11; w >= 0; w--) {
+    if (yc.l[w] != e[w]) { larger = yc.l[w] > e[w]; break; }
+  }
+  if (larger != (v.sign != 0)) y = y.neg();
+  // [r]P = O, r = the group order, by double-and-add from the top bit (host_bls12_381.hpp in_subgroup)
+  Xyzz<FpD> base, acc = Xyzz<FpD>::inf();
+  base.x = x; base.y = y; base.zz = FpD::one(); base.zzz = FpD::one();
+#pragma unroll 1
+  for (int b = 254; b >= 0; b--) {
+    acc = xyzz_dbl_u(acc);
+    if ((Bls12381Fr::P(b >> 5) >> (b & 31)) & 1u) xyzz_add_u(acc, base);
+  }
+  const bool ok = acc.is_inf();
+  store_words(o, ok ? x : FpD::zero());
+  store_words(o + FpD::WORDS, ok ? y : FpD::zero());
+  status[i] = ok ? 0 : 8;
+}
+
+// rp[k] = r^(k + 1) for k < n (the reference's powers skip r^0): square-and-multiply on k + 1 per thread
+__global__ void __launch_bounds__(VER_THREADS) k_ver_powers(const uint32_t* __restrict__ r_mont, size_t n, uint32_t* rp) {
+  const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  FrD r, acc = FrD::one();
+  load_words(r, r_mont);
+  const uint64_t e = k + 1;
+  for (int b = 63 - __clzll((long long)e); b >= 0; b--) {
+    acc = acc.sqr();
+    if ((e >> b) & 1) acc = acc * r;
+  }
+  store_words(rp + 8 * k, acc);
+}
+
+// The two scalar rows of the bank (M = n + U + 64 each): row A = (r^k, 0, 0), row B = (r^k h_k^64, sum of r^k per commitment, -I).
+// Thread t < n: proof t; n <= t < n + U: commitment t - n (its cells are com_list[com_start[i] .. com_start[i + 1])); the rest of
+// row A is zero; the last 64 entries of row B are written by k_ver_interp.
+__global__ void __launch_bounds__(VER_THREADS) k_ver_scalars(const uint32_t* rp, const uint32_t* __restrict__ cols,
+                                                             const uint32_t* __restrict__ com_start, const uint32_t* __restrict__ com_list,
+                                                             const uint32_t* __restrict__ tw, size_t n, size_t U, uint32_t* scalars) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t M = n + U + DAS_L;
+  if (t >= M) return;
+  uint32_t* a = scalars + 8 * t;
+  uint32_t* b = scalars + 8 * (M + t);
+  if (t < n) {
+    FrD v, h;
+    load_words_rw(v, rp + 8 * t);
+    load_words(h, tw + 8 * (DAS_L * brp7(cols[t])));   // h_k^64 = w128^brp7(c) = w8192^(64 brp7(c))
+    store_words(a, v);
+    store_words(b, v * h);
+  } else {
+    store_words(a, FrD::zero());
+    if (t < n + U) {
+      const size_t i = t - n;
+      FrD s = FrD::zero();
+      for (uint32_t q = com_start[i]; q < com_start[i + 1]; q++) {
+        FrD v;
+        load_words_rw(v, rp + 8 * (size_t)com_list[q]);
+        s = s + v;
+      }
+      store_words(b, s);
+    }
+  }
+}
+
+// One block of 64 threads per used column u (column col_id[u], cells col_list[col_start[u] .. col_start[u + 1])). Thread j: sum_k r^k
+// evals_k[j] (brp order within the cell); then the inverse NTT of 64 (brp in, natural out, DIT), scaled by 1/64 and h_c^-i,
+// h_c = w8192^brp7(c) (coset_ifft_rn): out[u * 64 + i].
+__global__ void __launch_bounds__(DAS_L) k_ver_columns(const uint32_t* cells, const uint32_t* rp, const uint32_t* __restrict__ col_id,
+                                                       const uint32_t* __restrict__ col_start, const uint32_t* __restrict__ col_list,
+                                                       const uint32_t* __restrict__ tw, uint32_t* out) {
+  __shared__ __align__(16) uint32_t s[DAS_L * 8];
+  const int j = threadIdx.x;
+  const size_t u = blockIdx.x;
+  FrD acc = FrD::zero();
+  for (uint32_t q = col_start[u]; q < col_start[u + 1]; q++) {
+    const size_t k = col_list[q];
+    FrD w, v;
+    load_words_rw(w, rp + 8 * k);
+    load_words_rw(v, cells + 8 * (k * DAS_L + j));
+    acc = acc + w * v;
+  }
+  store_words(s + 8 * j, acc);
+  __syncthreads();
+#pragma unroll 1
+  for (int lh = 0; lh < 6; lh++) {                    // span h = 2^lh; w_{2h}^jj = w8192^(jj * 4096 / h), inverse direction
+    const int h = 1 << lh;
+    if (j < DAS_L / 2) {
+      const int jj = j & (h - 1);
+      const int i0 = ((j >> lh) << (lh + 1)) + jj, i1 = i0 + h;
+      FrD a, c;
+      load_words_rw(a, s + 8 * i0);
+      load_words_rw(c, s + 8 * i1);
+      if (jj) {
+        FrD w;
+        load_words(w, tw + 8 * (8192 - (jj << (12 - lh))));
+        c = c * w;
+      }
+      store_words(s + 8 * i0, a + c);
+      store_words(s + 8 * i1, a - c);
+    }
+    __syncthreads();
+  }
+  FrD v, inv64, hi;
+  load_words_rw(v, s + 8 * j);
+  load_words(inv64, tw + 8 * DAS_TW_INV64);
+  load_words(hi, tw + 8 * ((8192 - (brp7(col_id[u]) * (uint32_t)j) % 8192) % 8192));
+  store_words(out + 8 * (u * DAS_L + j), v * inv64 * hi);
+}
+
+// 64 threads: -(sum over the used columns) -> the last 64 scalars of row B
+__global__ void __launch_bounds__(DAS_L) k_ver_interp(const uint32_t* colres, size_t used, size_t M, uint32_t* scalars) {
+  const int j = threadIdx.x;
+  FrD s = FrD::zero();
+  for (size_t u = 0; u < used; u++) {
+    FrD v;
+    load_words_rw(v, colres + 8 * (u * DAS_L + j));
+    s = s + v;
+  }
+  store_words(scalars + 8 * (M + M - DAS_L + j), s.neg());
+}
+
+int verify_device(const void* d_tw, const void* d_mono, const VerifyBatch& vb, const std::function<void()>& overlap,
+                  const std::function<int(const uint8_t*)>& decide, const std::function<void(uint64_t*)>& challenge,
+                  host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times) {
+  using C = Bls12381G1;
+  using HP = host::HXyzz<typename C::H>;
+  EngineLease lease = acquire_engine();
+  Engine& E = *lease.e;
+  cudaStream_t s = E.compute();
+  const size_t n = vb.n, U = vb.U, npts = n + U, M = npts + DAS_L, used = vb.used_cols;
+  const uint32_t* tw = (const uint32_t*)d_tw;
+  constexpr size_t AFF = 2 * FpD::WORDS * 4;
+  // device layout of ver_in: points in | cells | column ids | column starts | column lists | commitment starts | commitment lists | r
+  const size_t in_bytes = npts * sizeof(VerifyPoint), cell_bytes = n * (size_t)DAS_L * 32;
+  const size_t o_cells = (in_bytes + 255) & ~(size_t)255;
+  const size_t o_idx = o_cells + cell_bytes;
+  const size_t idx_words = used + (used + 1) + n + (U + 1) + n + n;
+  const size_t o_r = (o_idx + idx_words * 4 + 255) & ~(size_t)255;
+  E.ver_in.ensure(o_r + 64);
+  E.ver_pts.ensure(M * AFF);
+  E.ver_aux.ensure(npts + n * 32 + used * DAS_L * 32 + 512);
+  char* base = (char*)E.ver_in.ptr;
+  uint32_t* d_cells = (uint32_t*)(base + o_cells);
+  uint32_t* d_idx = (uint32_t*)(base + o_idx);
+  uint32_t* d_col_id = d_idx;
+  uint32_t* d_col_start = d_col_id + used;
+  uint32_t* d_col_list = d_col_start + used + 1;
+  uint32_t* d_com_start = d_col_list + n;
+  uint32_t* d_com_list = d_com_start + U + 1;
+  uint32_t* d_cols = d_com_list + n;
+  uint32_t* d_r = (uint32_t*)(base + o_r);
+  uint8_t* d_status = (uint8_t*)E.ver_aux.ptr;
+  uint32_t* d_rp = (uint32_t*)((char*)E.ver_aux.ptr + ((npts + 255) & ~(size_t)255));
+  uint32_t* d_colres = d_rp + 8 * n;
+
+  // 1. decode (and the cells behind it), statuses back; the host checks the cells and hashes meanwhile
+  B200_CUDA_CHECK(cudaMemcpyAsync(base, vb.points, in_bytes, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[7], s));
+  k_ver_decode<<<(unsigned)((npts + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>((const VerifyPoint*)base, npts,
+                                                                                           (uint32_t*)E.ver_pts.ptr, d_status);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
+  E.ensure_host(npts);
+  B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, d_status, npts, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_cells, vb.cells, cell_bytes, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_idx, vb.index_words, idx_words * 4, cudaMemcpyHostToDevice, s));
+  overlap();
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  if (times) {
+    *times = VerifyTimes();
+    cudaEventElapsedTime(&times->ms_decode, E.ev[7], E.ev[8]);
+  }
+  const int st = decide((const uint8_t*)E.h_result);
+  if (st != 0) return st;
+
+  // 2. scalars
+  uint64_t r[4];
+  challenge(r);
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_r, r, 32, cudaMemcpyHostToDevice, s));
+  E.d_scalars.ensure(2 * M * 32 + 16);
+  uint32_t* sc = (uint32_t*)E.d_scalars.ptr;
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[11], s));
+  k_kzg_parse<<<(unsigned)((n * DAS_L + 255) / 256), 256, 0, s>>>(d_cells, n * DAS_L);
+  k_ver_powers<<<(unsigned)((n + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>(d_r, n, d_rp);
+  k_ver_scalars<<<(unsigned)((M + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>(d_rp, d_cols, d_com_start, d_com_list, tw, n, U, sc);
+  k_ver_columns<<<(unsigned)used, DAS_L, 0, s>>>(d_cells, d_rp, d_col_id, d_col_start, d_col_list, tw, d_colres);
+  k_ver_interp<<<1, DAS_L, 0, s>>>(d_colres, used, M, sc);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpyAsync((char*)E.ver_pts.ptr + npts * AFF, d_mono, DAS_L * AFF, cudaMemcpyDeviceToDevice, s));
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[12], s));
+
+  // 3. the bank of 2 MSMs over the shared point set
+  E.stats.ms_h2d = 0;
+  HP res[2] = {HP::inf(), HP::inf()};
+  msm_device<C>(E, sc, E.ver_pts.ptr, M, /*fr_mont=*/true, 0, 0, -1, nullptr, 0, /*batch=*/2, /*point_sets=*/1, res);
+  thread_stats() = E.stats;
+  out[0] = res[0];
+  out[1] = res[1];
+  if (times) {
+    cudaEventElapsedTime(&times->ms_fr, E.ev[11], E.ev[12]);
+    times->ms_msm = E.collect_timing ? E.stats.ms_total : 0.f;
+  }
+  return 0;
+}
+
+}  // namespace kzg
+}  // namespace b200

@@ -403,6 +403,7 @@ class EthKzgContext:
         rc = _lib.load().ctt_b200_eth_kzg_context_load_peerdas(self._h, _buf(srs_monomial_compressed))
         if rc != 0:
             raise ValueError(rc)
+        self._peerdas_loaded = True
 
     def _split(self, cells_raw, proofs_raw, n):
         c, k = self.BYTES_PER_CELL, self.CELLS_PER_EXT_BLOB
@@ -486,6 +487,51 @@ class EthKzgContext:
             raise ValueError(rc, failed.value)
         c, p = self._split(out_cells.raw, out_proofs.raw, n)
         return list(zip(c, p))
+
+    # EIP-7594 batch verification (reference constantine/eth_eip7594_peerdas.nim:509-619)
+    def load_g2_setup(self, srs_monomial_g2_compressed):
+        """One-time: the 65 monomial G2 points of the trusted setup (96-byte compressed, file order), decoded and checked.
+        Raises ValueError(status) at the first bad point."""
+        self._check_len("srs_monomial_g2_compressed", srs_monomial_g2_compressed, 65 * 96)
+        rc = _lib.load().ctt_b200_eth_kzg_context_load_g2_setup(self._h, _buf(srs_monomial_g2_compressed))
+        if rc != 0:
+            raise ValueError(rc)
+        self._g2_loaded = True
+
+    def verify_cell_kzg_proof_batch(self, commitments, cell_indices, cells, proofs, secure_random_bytes=bytes(32)) -> bool:
+        """True when every cell k belongs, at column cell_indices[k], to the blob committed to by commitments[k] (proof proofs[k]);
+        False when the batch does not verify. Needs load_peerdas and load_g2_setup (else RuntimeError, so False always means "does
+        not verify"). Lists of unequal length or items of the wrong size raise ValueError(str); a status from the library (2, 4-8)
+        raises ValueError(status). secure_random_bytes: 32 bytes; when they reduce to zero the Fiat-Shamir challenge is used."""
+        if not (getattr(self, "_peerdas_loaded", False) and getattr(self, "_g2_loaded", False)):
+            raise RuntimeError("verify_cell_kzg_proof_batch needs load_peerdas and load_g2_setup")
+        commitments, cells, proofs = [bytes(c) for c in commitments], [bytes(c) for c in cells], [bytes(p) for p in proofs]
+        cell_indices = [int(i) for i in cell_indices]
+        n = len(cells)
+        if not len(commitments) == len(cell_indices) == n == len(proofs):
+            raise ValueError(f"{len(commitments)} commitments, {len(cell_indices)} cell indices, {n} cells and {len(proofs)} proofs")
+        for c in commitments:
+            self._check_len("commitment", c, 48)
+        for p in proofs:
+            self._check_len("proof", p, 48)
+        for c in cells:
+            self._check_len("cell", c, self.BYTES_PER_CELL)
+        self._check_len("secure_random_bytes", secure_random_bytes, 32)
+        idx = (ctypes.c_uint64 * max(1, n))(*cell_indices)
+        rc = _lib.load().ctt_b200_eth_kzg_verify_cell_kzg_proof_batch(self._h, _buf(b"".join(commitments) or b"\0"), idx,
+                                                                      _buf(b"".join(cells) or b"\0"), _buf(b"".join(proofs) or b"\0"),
+                                                                      n, _buf(bytes(secure_random_bytes)))
+        if rc not in (0, 1):
+            raise ValueError(rc)
+        return rc == 0
+
+    @staticmethod
+    def last_verify_timing() -> dict:
+        """Host checks + challenge, device decode, scalar kernels, bank MSM (CUDA events) and host pairing time (ms) of the calling
+        thread's last verify_cell_kzg_proof_batch."""
+        v = [ctypes.c_float(0) for _ in range(5)]
+        _lib.load().ctt_b200_eth_kzg_last_verify_timing(*[ctypes.byref(x) for x in v])
+        return dict(zip(("ms_host", "ms_decode", "ms_fr", "ms_msm", "ms_pairing"), (x.value for x in v)))
 
     @staticmethod
     def last_das_timing() -> dict:

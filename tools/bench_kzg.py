@@ -3,8 +3,12 @@
 the window table, and the split of one proof call (host checks + SHA-256, k_kzg_* kernels, MSM). The PeerDAS leg: the one-time
 load_peerdas, compute_cells_and_kzg_proofs as n single calls against one batched call, and the split of a call (host, Fr kernels,
 bank MSM with its engine phases, EC FFTs). The recovery leg: recover_cells_and_kzg_proofs with 64 seeded random cells missing per
-blob, as n single calls against one batched call, and the same split. Prints one JSON line.
-python tools/bench_kzg.py [--reps R] [--sizes 1,6,9,32,128] [--das-sizes 1,6,21,72] [--rec-sizes 1,6,21,72]"""
+blob, as n single calls against one batched call, and the same split. The verify leg: verify_cell_kzg_proof_batch over n cells of 72
+random blobs (n = 128, 6 x 128, 21 x 128, 72 x 128 shuffled; one column of 72; 8 columns of 72), with the Fiat-Shamir challenge and with
+caller-supplied random bytes: the median per call and its split (host checks + challenge, device decode, scalar kernels, bank MSM,
+host pairing). Prints one JSON line.
+python tools/bench_kzg.py [--reps R] [--sizes 1,6,9,32,128] [--das-sizes 1,6,21,72] [--rec-sizes 1,6,21,72] [--verify-sizes 1,6,21,72]
+                          [--only verify]"""
 import argparse
 import json
 import os
@@ -87,16 +91,51 @@ def recovery(ctx, sizes, reps):
     return r
 
 
+def verify(ctx, sizes, reps):
+    """Needs load_peerdas (the PeerDAS leg or the caller loads it). sizes: numbers of 128-cell rows."""
+    ctx.load_g2_setup(np.load(os.path.join(ROOT, "tests", "golden", "peerdas_verify_kat.npz"))["srs_monomial_g2_compressed"].tobytes())
+    blobs = random_blobs(72, 7597)
+    cms = ctx.blobs_to_kzg_commitments(blobs)
+    full = ctx.compute_cells_and_kzg_proofs_batch(blobs)
+    rnd = random.Random(7597)
+    every = [(b, c) for b in range(72) for c in range(128)]
+    rnd.shuffle(every)
+    shapes = {f"cells{128 * n}": every[:128 * n] for n in sizes}
+    shapes["col1x72"] = [(b, 77) for b in range(72)]
+    shapes["col8x72"] = [(b, c) for c in range(0, 128, 16) for b in range(72)]
+    r = {}
+    for name, picks in shapes.items():
+        a = ([cms[b] for b, _ in picks], [c for _, c in picks], [full[b][0][c] for b, c in picks], [full[b][1][c] for b, c in picks])
+        for path, rb in (("fs", bytes(32)), ("rand", bytes(range(1, 33)))):
+            assert ctx.verify_cell_kzg_proof_batch(*a, secure_random_bytes=rb)
+            splits = []
+            ctx.verify_cell_kzg_proof_batch(*a, secure_random_bytes=rb)
+            for _ in range(reps):
+                t0 = time.perf_counter()
+                ctx.verify_cell_kzg_proof_batch(*a, secure_random_bytes=rb)
+                splits.append({"wall_ms": (time.perf_counter() - t0) * 1e3, **ctx.last_verify_timing()})
+            r[f"{name}_{path}_ms"] = {k: round(statistics.median(s[k] for s in splits), 3) for k in splits[0]}
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--sizes", default="1,6,9,32,128")
     ap.add_argument("--das-sizes", default="1,6,21,72")
     ap.add_argument("--rec-sizes", default="1,6,21,72")
+    ap.add_argument("--verify-sizes", default="1,6,21,72")
+    ap.add_argument("--only", default="", help="'verify': only the verify leg (after load_peerdas)")
     a = ap.parse_args()
     sizes = [int(s) for s in a.sizes.split(",")]
     srs = np.load(os.path.join(ROOT, "tests", "golden", "kzg_commit_kat.npz"))["srs_lagrange_brp_compressed"].tobytes()
     ctx = M.EthKzgContext(srs, compressed=True)
+    vsizes = [int(s) for s in a.verify_sizes.split(",")]
+    if a.only == "verify":
+        ctx.load_peerdas(np.load(os.path.join(ROOT, "tests", "golden", "peerdas_kat.npz"))["srs_monomial_compressed"].tobytes())
+        print(json.dumps({"gpu": bench.gpu_identity(0), "reps": a.reps, "verify": verify(ctx, vsizes, a.reps)}), flush=True)
+        ctx.delete()
+        return
     blobs = random_blobs(max(sizes), 4844)
     cms = ctx.blobs_to_kzg_commitments(blobs)
     out = {"gpu": bench.gpu_identity(0), "reps": a.reps, "modes": {}}
@@ -121,6 +160,7 @@ def main():
         out["modes"][mode] = r
     out["peerdas"] = peerdas(ctx, [int(s) for s in a.das_sizes.split(",")], a.reps)
     out["recovery"] = recovery(ctx, [int(s) for s in a.rec_sizes.split(",")], a.reps)
+    out["verify"] = verify(ctx, vsizes, a.reps)
     ctx.delete()
     print(json.dumps(out), flush=True)
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Small MSMs on every curve and a 2-blob PeerDAS recovery, meant to run under compute-sanitizer (memcheck / racecheck):
+"""Small MSMs on every curve, a 2-blob PeerDAS recovery and a 40-cell batch verification, meant to run under compute-sanitizer (memcheck / racecheck):
    compute-sanitizer --tool racecheck python tools/sanitize_small.py"""
 import os, random, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -31,4 +31,11 @@ ctx.load_peerdas(das["srs_monomial_compressed"].tobytes())
 full = ctx.compute_cells_and_kzg_proofs_batch([bytes(commit["blobs"][1]), bytes(commit["blobs"][2])])
 items = [(idx, [cells[i] for i in idx]) for idx, (cells, _) in zip((list(range(0, 128, 2)), sorted(r.sample(range(128), 100))), full)]
 print("recovery 2 blobs", "OK" if ctx.recover_cells_and_kzg_proofs_batch(items) == full else "MISMATCH", flush=True)
+# a 40-cell verify_cell_kzg_proof_batch over both blobs (decode, scalar and column kernels, the bank MSM)
+ctx.load_g2_setup(np.load(os.path.join(g, "peerdas_verify_kat.npz"))["srs_monomial_g2_compressed"].tobytes())
+cms = ctx.blobs_to_kzg_commitments([bytes(commit["blobs"][1]), bytes(commit["blobs"][2])])
+picks = [(r.randrange(2), r.randrange(128)) for _ in range(40)]
+ok = ctx.verify_cell_kzg_proof_batch([cms[b] for b, _ in picks], [c for _, c in picks], [full[b][0][c] for b, c in picks],
+                                     [full[b][1][c] for b, c in picks])
+print("verify 40 cells", "OK" if ok else "MISMATCH", flush=True)
 ctx.delete()
