@@ -134,6 +134,12 @@ def load():
     lib.ctt_b200_eth_kzg_context_load_g2_setup.restype = ci
     lib.ctt_b200_eth_kzg_verify_cell_kzg_proof_batch.argtypes = [vp, vp, vp, vp, vp, sz, vp]
     lib.ctt_b200_eth_kzg_verify_cell_kzg_proof_batch.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_kzg_verify_kzg_proof.argtypes = [vp, vp, vp, vp, vp]
+    lib.ctt_b200_eth_kzg_verify_kzg_proof.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_kzg_verify_blob_kzg_proof.argtypes = [vp, vp, vp, vp]
+    lib.ctt_b200_eth_kzg_verify_blob_kzg_proof.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_kzg_verify_blob_kzg_proof_batch.argtypes = [vp, vp, vp, vp, sz, vp]
+    lib.ctt_b200_eth_kzg_verify_blob_kzg_proof_batch.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_kzg_last_verify_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 5
     lib.ctt_b200_eth_kzg_last_verify_timing.restype = None
     lib.ctt_threadpool_new.argtypes = [ci]

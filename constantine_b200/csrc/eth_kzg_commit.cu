@@ -247,6 +247,109 @@ static G1Aff xyzz_affine(const HP& p) {
   return a;
 }
 
+// ---- EIP-4844 verification ---------------------------------------------------------------------------------------------------
+// The G1 generator, 48-byte compressed: the last point of the blob entries' MSM point set, and [y]G1 of verify_kzg_proof
+static const uint8_t G1_GENERATOR[48] = {
+    0x97, 0xf1, 0xd3, 0xa7, 0x31, 0x97, 0xd7, 0x94, 0x26, 0x95, 0x63, 0x8c, 0x4f, 0xa9, 0xac, 0x0f, 0xc3, 0x68, 0x8c, 0x4f, 0x97, 0x74, 0xb9, 0x05,
+    0xa1, 0x4e, 0x3a, 0x3f, 0x17, 0x1b, 0xac, 0x58, 0x6c, 0x55, 0xe8, 0x3f, 0xf9, 0x7a, 0x1a, 0xef, 0xfb, 0x3a, 0xf0, 0x0a, 0xdb, 0x22, 0xc6, 0xbb};
+
+static HP affine_xyzz(const Fp& x, const Fp& y) {
+  if (x.is_zero() && y.is_zero()) return HP::inf();
+  HP p; p.x = x; p.y = y; p.zz = Fp::one(); p.zzz = Fp::one();
+  return p;
+}
+
+// [k]P by double-and-add from the top bit (k canonical, < r); P affine, infinity as (0, 0)
+static HP host_scalar_mul(const Fp& x, const Fp& y, const uint64_t k[4]) {
+  const HP p = affine_xyzz(x, y);
+  HP acc = HP::inf();
+  for (int b = 254; b >= 0; b--) {
+    acc = host::xyzz_dbl(acc);
+    if ((k[b >> 6] >> (b & 63)) & 1) acc = host::xyzz_add(acc, p);
+  }
+  return acc;
+}
+
+// e(P1, Q1) e(P2, -G2) = 1 (both verification families), timed into the verification timing
+static unsigned char pairing_neg_g2(const Context* k, const HP& p1, const G2Aff& q1, const HP& p2, VerifyTiming& tm) {
+  const auto t0 = std::chrono::steady_clock::now();
+  G2Aff neg_g2 = k->g2[0];
+  neg_g2.y = neg_g2.y.neg();
+  const bool ok = pairing_check(xyzz_affine(p1), q1, xyzz_affine(p2), neg_g2);
+  tm.ms_pairing = (float)ms_since(t0);
+  return (unsigned char)(ok ? Success : VerificationFailure);
+}
+
+// verify_blob_kzg_proof (n = 1, r = 1, the proof checked before the blob) and verify_blob_kzg_proof_batch (per index: commitment, blob,
+// proof; r from secure_random_bytes or the challenges). The per-point work runs on the device (verify_blob_device); the host checks the
+// blob elements and computes the challenges z_i while the device decodes the points.
+static unsigned char verify_blobs(const Context* k, const uint8_t* blobs, const uint8_t* commitments, const uint8_t* proofs, size_t n,
+                                  const uint8_t* secure_random_bytes) {
+  const bool single = secure_random_bytes == nullptr;
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<VerifyPoint> pts(2 * n + 1);
+  for (size_t i = 0; i < n; i++) {
+    pts[i] = verify_point(commitments + 48 * i);
+    pts[n + i] = verify_point(proofs + 48 * i);
+  }
+  pts[2 * n] = verify_point(G1_GENERATOR);
+  BlobVerifyBatch vb;
+  vb.n = n; vb.points = pts.data(); vb.blobs = blobs;
+
+  double ms_host = ms_since(t0);
+  std::vector<int> blob_status(n, Success);
+  std::vector<OpeningArgs> args(n);
+  std::vector<Fr> zm(n);
+  uint64_t r_mont[4] = {0, 0, 0, 0};
+  auto overlap = [&] {
+    const auto t1 = std::chrono::steady_clock::now();
+    parallel_for(n, [&](size_t j) {
+      blob_status[j] = check_blob(blobs + BYTES_PER_BLOB * j, nullptr);
+      if (blob_status[j] != Success) return;
+      uint64_t zc[4];
+      fiat_shamir_challenge(zc, blobs + BYTES_PER_BLOB * j, commitments + 48 * j);
+      zm[j] = fr_to_mont(zc);
+      args[j] = opening_args(k, zc);
+    });
+    bool blobs_ok = true;
+    for (size_t j = 0; j < n; j++) blobs_ok = blobs_ok && blob_status[j] == Success;
+    if (blobs_ok) {
+      Fr rm = Fr::one();
+      if (!single) {
+        uint64_t r[4];
+        blob_batch_blinding(r, secure_random_bytes, zm.data(), n);
+        rm = fr_to_mont(r);
+      }
+      memcpy(r_mont, rm.l, 32);
+    }
+    ms_host += ms_since(t1);
+  };
+  auto decide = [&](const uint8_t* st) -> int {
+    for (size_t i = 0; i < n; i++) {
+      if (st[i]) return st[i];
+      if (single) {
+        if (st[n + i]) return st[n + i];
+        if (blob_status[i] != Success) return blob_status[i];
+      } else {
+        if (blob_status[i] != Success) return blob_status[i];
+        if (st[n + i]) return st[n + i];
+      }
+    }
+    return Success;
+  };
+  HP res[2];
+  VerifyTimes times;
+  const int st = verify_blob_device(k->d_roots, vb, overlap, decide, args.data(), r_mont, res, &times);
+  VerifyTiming& tm = last_verify_timing();
+  tm = VerifyTiming();
+  tm.ms_host = (float)ms_host;
+  tm.ms_decode = times.ms_decode;
+  if (st != Success) return (unsigned char)st;
+  tm.ms_fr = times.ms_fr;
+  tm.ms_msm = times.ms_msm;
+  return pairing_neg_g2(k, res[0], k->g2[1], res[1], tm);
+}
+
 }  // namespace kzg
 }  // namespace b200
 
@@ -540,16 +643,66 @@ unsigned char ctt_b200_eth_kzg_verify_cell_kzg_proof_batch(const ctt_b200_eth_kz
   if (st != Success) return (unsigned char)st;
   tm.ms_fr = times.ms_fr;
   tm.ms_msm = times.ms_msm;
-  const auto t2 = std::chrono::steady_clock::now();
-  G2Aff neg_g2 = k->g2[0];
-  neg_g2.y = neg_g2.y.neg();
-  const bool ok = pairing_check(xyzz_affine(res[0]), k->g2[DAS_L_G2 - 1], xyzz_affine(res[1]), neg_g2);
-  tm.ms_pairing = (float)ms_since(t2);
-  return (unsigned char)(ok ? Success : VerificationFailure);
+  return pairing_neg_g2(k, res[0], k->g2[DAS_L_G2 - 1], res[1], tm);
 }
 
-// the last verify_cell_kzg_proof_batch call of the calling thread: host checks + challenge, the device decode, the scalar kernels and
-// the bank MSM (CUDA events), and the host pairing check
+// reference ctt_eth_kzg_verify_kzg_proof (ethereum_eip4844_kzg.nim:380-407); needs load_g2_setup. Host only: two points, a few scalar
+// multiplications and one pairing check. Checks in the reference's order: commitment (5-8), z < r (4), y < r (4), proof (5-8).
+unsigned char ctt_b200_eth_kzg_verify_kzg_proof(const ctt_b200_eth_kzg_context* ctx, const unsigned char commitment[48],
+                                                const unsigned char z[32], const unsigned char y[32], const unsigned char proof[48]) {
+  const Context* k = reinterpret_cast<const Context*>(ctx);
+  if (!k || k->g2.size() != DAS_L_G2) return (unsigned char)VerificationFailure;
+  if (!commitment || !z || !y || !proof) return (unsigned char)InputsLengthsMismatch;
+  const auto t0 = std::chrono::steady_clock::now();
+  VerifyTiming& tm = last_verify_timing();
+  tm = VerifyTiming();
+  G1Aff c, pi, g;
+  int rc = decompress_g1(c.x, c.y, commitment);
+  if (rc == Success && !c.inf() && !in_subgroup(c.x, c.y)) rc = EccPointNotInSubgroup;
+  if (rc != Success) return (unsigned char)rc;
+  uint64_t zc[4], yc[4];
+  be32_to_limbs(zc, z);
+  if (geq_order(zc)) return (unsigned char)ScalarLargerThanCurveOrder;
+  be32_to_limbs(yc, y);
+  if (geq_order(yc)) return (unsigned char)ScalarLargerThanCurveOrder;
+  rc = decompress_g1(pi.x, pi.y, proof);
+  if (rc == Success && !pi.inf() && !in_subgroup(pi.x, pi.y)) rc = EccPointNotInSubgroup;
+  if (rc != Success) return (unsigned char)rc;
+  decompress_g1(g.x, g.y, G1_GENERATOR);
+  // e(pi, [tau]G2) e(C + [z]pi - [y]G1, -G2) = 1
+  const HP yg = host_scalar_mul(g.x, g.y.neg(), yc);
+  const HP rhs = b200::host::xyzz_add(b200::host::xyzz_add(affine_xyzz(c.x, c.y), host_scalar_mul(pi.x, pi.y, zc)), yg);
+  tm.ms_host = (float)ms_since(t0);
+  return pairing_neg_g2(k, affine_xyzz(pi.x, pi.y), k->g2[1], rhs, tm);
+}
+
+// reference ctt_eth_kzg_verify_blob_kzg_proof (ethereum_eip4844_kzg.nim:449-485); needs load_g2_setup. Checks in the reference's order:
+// commitment (5-8), proof (5-8), every blob element < r (4).
+unsigned char ctt_b200_eth_kzg_verify_blob_kzg_proof(const ctt_b200_eth_kzg_context* ctx, const unsigned char* blob,
+                                                     const unsigned char commitment[48], const unsigned char proof[48]) {
+  const Context* k = reinterpret_cast<const Context*>(ctx);
+  if (!k || k->g2.size() != DAS_L_G2) return (unsigned char)VerificationFailure;
+  if (!blob || !commitment || !proof) return (unsigned char)InputsLengthsMismatch;
+  return verify_blobs(k, blob, commitment, proof, 1, nullptr);
+}
+
+// reference ctt_eth_kzg_verify_blob_kzg_proof_batch (ethereum_eip4844_kzg.nim:487-570); needs load_g2_setup. Checks per index, lowest
+// first: commitment (5-8), blob (4), proof (5-8); the first failing one is reported. r: secure_random_bytes reduced mod r when that is not
+// zero, else the hash of the opening challenges (blob_batch_blinding); the powers r^1 .. r^n weight the n openings.
+unsigned char ctt_b200_eth_kzg_verify_blob_kzg_proof_batch(const ctt_b200_eth_kzg_context* ctx, const unsigned char* blobs,
+                                                           const unsigned char* commitments, const unsigned char* proofs, size_t n,
+                                                           const unsigned char secure_random_bytes[32]) {
+  const Context* k = reinterpret_cast<const Context*>(ctx);
+  if (!k || k->g2.size() != DAS_L_G2) return (unsigned char)VerificationFailure;
+  if (n == 0) return (unsigned char)Success;
+  if (!blobs || !commitments || !proofs || !secure_random_bytes) return (unsigned char)InputsLengthsMismatch;
+  return verify_blobs(k, blobs, commitments, proofs, n, secure_random_bytes);
+}
+
+// the last verification of the calling thread, of either family (verify_cell_kzg_proof_batch, verify_kzg_proof, verify_blob_kzg_proof,
+// verify_blob_kzg_proof_batch): host checks + challenges, the device decode of the points, the scalar kernels (with the blobs' parse
+// and evaluation) and the bank MSM (CUDA events), and the host pairing check. verify_kzg_proof is host only: its point work is in
+// ms_host and its device phases are 0.
 void ctt_b200_eth_kzg_last_verify_timing(float* ms_host, float* ms_decode, float* ms_fr, float* ms_msm, float* ms_pairing) {
   const VerifyTiming& t = last_verify_timing();
   if (ms_host) *ms_host = t.ms_host;

@@ -175,6 +175,28 @@ inline void cell_batch_challenge(uint64_t r[4], const uint8_t* unique_commitment
   reduce_be32(r, digest);
 }
 
+// ---- blinding factor of verify_blob_kzg_proof_batch (reference ethereum_eip4844_kzg.nim:148-162 and 533-543) ---------------------
+// The caller's 32 bytes reduced mod r when that is not zero (getBatchBlindingFactor). Otherwise SHA-256("RCKZGBATCH___V1_" || the n
+// opening challenges as the reference holds them in memory), reduced mod r: each z_i as its Montgomery residue z_i 2^256 mod r, four
+// little-endian 64-bit limbs. Returns true when the caller's bytes were used.
+inline bool blob_batch_blinding(uint64_t r[4], const uint8_t secure_random_bytes[32], const Fr* z_mont, size_t n) {
+  reduce_be32(r, secure_random_bytes);
+  if (r[0] | r[1] | r[2] | r[3]) return true;
+  static const char DOMAIN[] = "RCKZGBATCH___V1_";
+  Sha256 s;
+  s.update((const uint8_t*)DOMAIN, 16);
+  for (size_t i = 0; i < n; i++) {
+    uint8_t le[32];
+    for (int limb = 0; limb < 4; limb++)
+      for (int b = 0; b < 8; b++) le[8 * limb + b] = (uint8_t)(z_mont[i].l[limb] >> (8 * b));
+    s.update(le, 32);
+  }
+  uint8_t digest[32];
+  s.finish(digest);
+  reduce_be32(r, digest);
+  return false;
+}
+
 // ---- evaluation domain (reference commitments_setups/ethereum_kzg_srs.nim:389-394) --------------------------------------
 // roots[i] = w^brp(i), w = 7^((r - 1) / 4096), Montgomery form, brp = 12-bit reversal
 inline uint32_t reverse_bits12(uint32_t i) {

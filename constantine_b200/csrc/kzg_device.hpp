@@ -111,5 +111,23 @@ int verify_device(const void* d_tw, const void* d_mono, const VerifyBatch& vb, c
                   const std::function<int(const uint8_t*)>& decide, const std::function<void(uint64_t*)>& challenge,
                   host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times);
 
+// ---- EIP-4844 blob verification (verify_kernels.cuh) -------------------------------------------------------------------------
+// The inputs of verify_blob_kzg_proof[_batch] after the host's byte-level checks. points: 2n + 1 entries, the n commitments, the n
+// proofs, then the G1 generator; blobs: n x 131072 bytes as given.
+struct BlobVerifyBatch {
+  size_t n = 0;
+  const VerifyPoint* points = nullptr;
+  const uint8_t* blobs = nullptr;
+};
+
+// One engine lease and stream, as verify_device. Uploads and decodes the points, uploads and parses the blobs, runs `overlap` on the host
+// (the blob checks, the challenges z_i and r) while the device works, synchronises and calls `decide` with the per-point statuses; a
+// non-zero result is returned as it is. Otherwise args (n opening points) and r_mont (Fr Montgomery, 4 limbs), both filled by `overlap`,
+// are uploaded; k_ver_powers (r^1 .. r^n), k_kzg_eval (y_i = p_i(z_i)), k_kzg_ver_scalars and the bank of 2 MSMs over the decoded points
+// give out[0] = sum r^i pi_i and out[1] = sum r^i C_i + sum r^i z_i pi_i - [sum r^i y_i]G1 (raw XYZZ). d_roots: the context's domain.
+int verify_blob_device(const void* d_roots, const BlobVerifyBatch& vb, const std::function<void()>& overlap,
+                       const std::function<int(const uint8_t*)>& decide, const OpeningArgs* args, const uint64_t* r_mont,
+                       host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times);
+
 }  // namespace kzg
 }  // namespace b200

@@ -11,6 +11,8 @@
 //      shift h_c = w8192^brp7(c)), k_ver_interp (the column results summed and negated into row B);
 //   3. the engine: a bank of 2 MSMs over one shared point set [proofs | unique commitments | [tau^j]G1, j < 64].
 // The pairing check is host code (host_pairing.hpp). tests/peerdas_verify_exact.py computes the same scalars in Python.
+// The EIP-4844 blob verification (verify_blob_device, at the end) reuses k_ver_decode, k_kzg_parse and k_ver_powers and adds the blob
+// evaluation k_kzg_eval and its scalar kernel; tests/kzg_verify_exact.py computes its scalars.
 // Included by inst_bls12_381_g1.cu only, next to the engine instantiation it runs.
 #pragma once
 #include "peerdas_kernels.cuh"
@@ -264,6 +266,183 @@ int verify_device(const void* d_tw, const void* d_mono, const VerifyBatch& vb, c
   out[1] = res[1];
   if (times) {
     cudaEventElapsedTime(&times->ms_fr, E.ev[11], E.ev[12]);
+    times->ms_msm = E.collect_timing ? E.stats.ms_total : 0.f;
+  }
+  return 0;
+}
+
+// ---- EIP-4844 verify_blob_kzg_proof[_batch] (reference ethereum_eip4844_kzg.nim:449-570, commitments/kzg_parallel.nim:80-120) ----
+// e(sum r^i pi_i, [tau]G2) e(sum r^i C_i + sum r^i z_i pi_i - [sum r^i y_i]G1, -G2) = 1 over the point set [C | pi | G1] (M = 2n + 1).
+
+// y_b = p_b(z_b), one block per blob, no global scratch. Off the domain p(z) = f sum_i w_i p_i / (w_i - z) with
+// w_i / (w_i - z) = 1 + z / (w_i - z), so each thread keeps S = sum p_i and sum p_i / (w_i - z) as a fraction N / D (N' = N d + p D,
+// D' = D d, d = w_i - z: three multiplications per element); the block adds S and the fractions pairwise in shared memory and thread 0
+// inverts the one denominator: y = f (S + z N / D). For z = w_m, y = p_m (as in k_kzg_quotient).
+__global__ void __launch_bounds__(KZG_THREADS) k_kzg_eval(const uint32_t* __restrict__ poly, const uint32_t* __restrict__ roots,
+                                                         const OpeningArgs* __restrict__ args, uint32_t* y_out) {
+  __shared__ __align__(16) uint32_t red[3 * KZG_THREADS * 8];
+  const int t = threadIdx.x;
+  const size_t b = blockIdx.x;
+  const uint32_t* p = poly + b * (size_t)KZG_N * 8;
+  const int m = args[b].m;
+  if (m >= 0) {                                       // the same for the whole block
+    if (t == 0) {
+      FrD pm;
+      load_words(pm, p + 8 * m);
+      store_words(y_out + 8 * b, pm);
+    }
+    return;
+  }
+  FrD z;
+#pragma unroll
+  for (int w = 0; w < 8; w++) z.l[w] = args[b].z[w];
+  FrD S = FrD::zero(), num = FrD::zero(), den = FrD::one();
+#pragma unroll 1
+  for (int k = 0; k < KZG_RUN; k++) {
+    const int i = k * KZG_THREADS + t;
+    FrD w, pi;
+    load_words(w, roots + 8 * i);
+    load_words(pi, p + 8 * i);
+    const FrD d = w - z;
+    S = S + pi;
+    num = num * d + pi * den;
+    den = den * d;
+  }
+  uint32_t* rs = red;
+  uint32_t* rn = red + KZG_THREADS * 8;
+  uint32_t* rd = red + 2 * KZG_THREADS * 8;
+  store_words(rs + 8 * t, S);
+  store_words(rn + 8 * t, num);
+  store_words(rd + 8 * t, den);
+  __syncthreads();
+#pragma unroll 1
+  for (int s = KZG_THREADS / 2; s > 0; s >>= 1) {
+    if (t < s) {
+      FrD s0, s1, n0, n1, d0, d1;
+      load_words_rw(s0, rs + 8 * t);
+      load_words_rw(s1, rs + 8 * (t + s));
+      load_words_rw(n0, rn + 8 * t);
+      load_words_rw(n1, rn + 8 * (t + s));
+      load_words_rw(d0, rd + 8 * t);
+      load_words_rw(d1, rd + 8 * (t + s));
+      store_words(rs + 8 * t, s0 + s1);
+      store_words(rn + 8 * t, n0 * d1 + n1 * d0);
+      store_words(rd + 8 * t, d0 * d1);
+    }
+    __syncthreads();
+  }
+  if (t == 0) {
+    FrD s0, n0, d0, f;
+    load_words_rw(s0, rs);
+    load_words_rw(n0, rn);
+    load_words_rw(d0, rd);
+#pragma unroll
+    for (int w = 0; w < 8; w++) f.l[w] = args[b].f[w];
+    store_words(y_out + 8 * b, f * (s0 + z * n0 * fe_inverse(d0)));
+  }
+}
+
+// The two scalar rows of the bank (M = 2n + 1 each) in one block: row A = (0 | r^i | 0), row B = (r^i | r^i z_i | -sum r^i y_i); the
+// sum over the blobs is a block reduction.
+__global__ void __launch_bounds__(KZG_THREADS) k_kzg_ver_scalars(const uint32_t* rp, const OpeningArgs* __restrict__ args,
+                                                                const uint32_t* y, size_t n, uint32_t* scalars) {
+  __shared__ __align__(16) uint32_t red[KZG_THREADS * 8];
+  const size_t M = 2 * n + 1;
+  FrD s = FrD::zero();
+#pragma unroll 1
+  for (size_t i = threadIdx.x; i < n; i += KZG_THREADS) {
+    FrD r, z, yi;
+    load_words_rw(r, rp + 8 * i);
+    load_words_rw(yi, y + 8 * i);
+#pragma unroll
+    for (int w = 0; w < 8; w++) z.l[w] = args[i].z[w];
+    store_words(scalars + 8 * i, FrD::zero());
+    store_words(scalars + 8 * (n + i), r);
+    store_words(scalars + 8 * (M + i), r);
+    store_words(scalars + 8 * (M + n + i), r * z);
+    s = s + r * yi;
+  }
+  const FrD sum = kzg_block_sum(s, red);
+  if (threadIdx.x == 0) {
+    store_words(scalars + 8 * (2 * n), FrD::zero());
+    store_words(scalars + 8 * (M + 2 * n), sum.neg());
+  }
+}
+
+int verify_blob_device(const void* d_roots, const BlobVerifyBatch& vb, const std::function<void()>& overlap,
+                       const std::function<int(const uint8_t*)>& decide, const OpeningArgs* args, const uint64_t* r_mont,
+                       host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times) {
+  using C = Bls12381G1;
+  using HP = host::HXyzz<typename C::H>;
+  EngineLease lease = acquire_engine();
+  Engine& E = *lease.e;
+  cudaStream_t s = E.compute();
+  const size_t n = vb.n, M = 2 * n + 1, elems = n * (size_t)KZG_N;
+  constexpr size_t AFF = 2 * FpD::WORDS * 4;
+  // ver_in: points in | opening points | r;  ver_aux: statuses | r^i | y_i;  kzg_poly: the blobs
+  const size_t in_bytes = M * sizeof(VerifyPoint);
+  const size_t o_args = (in_bytes + 255) & ~(size_t)255;
+  const size_t o_r = (o_args + n * sizeof(OpeningArgs) + 255) & ~(size_t)255;
+  const size_t o_rp = (M + 255) & ~(size_t)255;
+  E.ver_in.ensure(o_r + 64);
+  E.ver_pts.ensure(M * AFF);
+  E.ver_aux.ensure(o_rp + 2 * n * 32 + 256);
+  E.kzg_poly.ensure(elems * 32);
+  char* base = (char*)E.ver_in.ptr;
+  OpeningArgs* d_args = (OpeningArgs*)(base + o_args);
+  uint32_t* d_r = (uint32_t*)(base + o_r);
+  uint8_t* d_status = (uint8_t*)E.ver_aux.ptr;
+  uint32_t* d_rp = (uint32_t*)((char*)E.ver_aux.ptr + o_rp);
+  uint32_t* d_y = d_rp + 8 * n;
+  uint32_t* d_poly = (uint32_t*)E.kzg_poly.ptr;
+
+  // 1. decode, statuses back, the blobs up and parsed behind them; the host checks the blobs and hashes meanwhile
+  B200_CUDA_CHECK(cudaMemcpyAsync(base, vb.points, in_bytes, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[7], s));
+  k_ver_decode<<<(unsigned)((M + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>((const VerifyPoint*)base, M,
+                                                                                        (uint32_t*)E.ver_pts.ptr, d_status);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
+  E.ensure_host(M);
+  B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, d_status, M, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_poly, vb.blobs, elems * 32, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[9], s));
+  k_kzg_parse<<<(unsigned)((elems + 255) / 256), 256, 0, s>>>(d_poly, elems);   // an element >= r is refused below; no use is made of it
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[10], s));
+  overlap();
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  float ms_parse = 0;
+  if (times) {
+    *times = VerifyTimes();
+    cudaEventElapsedTime(&times->ms_decode, E.ev[7], E.ev[8]);
+    cudaEventElapsedTime(&ms_parse, E.ev[9], E.ev[10]);
+  }
+  const int st = decide((const uint8_t*)E.h_result);
+  if (st != 0) return st;
+
+  // 2. the evaluations and the scalars
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_args, args, n * sizeof(OpeningArgs), cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_r, r_mont, 32, cudaMemcpyHostToDevice, s));
+  E.d_scalars.ensure(2 * M * 32 + 16);
+  uint32_t* sc = (uint32_t*)E.d_scalars.ptr;
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[11], s));
+  k_ver_powers<<<(unsigned)((n + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>(d_r, n, d_rp);
+  k_kzg_eval<<<(unsigned)n, KZG_THREADS, 0, s>>>(d_poly, (const uint32_t*)d_roots, d_args, d_y);
+  k_kzg_ver_scalars<<<1, KZG_THREADS, 0, s>>>(d_rp, d_args, d_y, n, sc);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(E.ev[12], s));
+
+  // 3. the bank of 2 MSMs over the decoded points
+  E.stats.ms_h2d = 0;
+  HP res[2] = {HP::inf(), HP::inf()};
+  msm_device<C>(E, sc, E.ver_pts.ptr, M, /*fr_mont=*/true, 0, 0, -1, nullptr, 0, /*batch=*/2, /*point_sets=*/1, res);
+  thread_stats() = E.stats;
+  out[0] = res[0];
+  out[1] = res[1];
+  if (times) {
+    cudaEventElapsedTime(&times->ms_fr, E.ev[11], E.ev[12]);
+    times->ms_fr += ms_parse;
     times->ms_msm = E.collect_timing ? E.stats.ms_total : 0.f;
   }
   return 0;

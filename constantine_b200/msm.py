@@ -525,10 +525,58 @@ class EthKzgContext:
             raise ValueError(rc)
         return rc == 0
 
+    # EIP-4844 verification (reference constantine/ethereum_eip4844_kzg.nim:380-570). Same conventions as verify_cell_kzg_proof_batch;
+    # these need load_g2_setup only.
+    def _need_g2(self, name):
+        if not getattr(self, "_g2_loaded", False):
+            raise RuntimeError(f"{name} needs load_g2_setup")
+
+    def _verify_status(self, rc) -> bool:
+        if rc not in (0, 1):
+            raise ValueError(rc)
+        return rc == 0
+
+    def verify_kzg_proof(self, commitment, z, y, proof) -> bool:
+        """True when proof opens the commitment at z (32 big-endian bytes) to y (32 big-endian bytes); False when it does not."""
+        self._need_g2("verify_kzg_proof")
+        for name, b, n in (("commitment", commitment, 48), ("z", z, 32), ("y", y, 32), ("proof", proof, 48)):
+            self._check_len(name, b, n)
+        return self._verify_status(_lib.load().ctt_b200_eth_kzg_verify_kzg_proof(self._h, _buf(bytes(commitment)), _buf(bytes(z)),
+                                                                                  _buf(bytes(y)), _buf(bytes(proof))))
+
+    def verify_blob_kzg_proof(self, blob, commitment, proof) -> bool:
+        """True when proof opens the commitment at the Fiat-Shamir challenge of (blob, commitment) to the blob's value there."""
+        self._need_g2("verify_blob_kzg_proof")
+        self._check_len("blob", blob, self.BYTES_PER_BLOB)
+        self._check_len("commitment", commitment, 48)
+        self._check_len("proof", proof, 48)
+        return self._verify_status(_lib.load().ctt_b200_eth_kzg_verify_blob_kzg_proof(self._h, _buf(bytes(blob)), _buf(bytes(commitment)),
+                                                                                      _buf(bytes(proof))))
+
+    def verify_blob_kzg_proof_batch(self, blobs, commitments, proofs, secure_random_bytes=bytes(32)) -> bool:
+        """True when every (blob, commitment, proof) verifies, checked as one random linear combination in one device pass.
+        secure_random_bytes: 32 bytes; when they reduce to zero, r is derived from the opening challenges."""
+        self._need_g2("verify_blob_kzg_proof_batch")
+        blobs, commitments, proofs = [bytes(b) for b in blobs], [bytes(c) for c in commitments], [bytes(p) for p in proofs]
+        n = len(blobs)
+        if not len(commitments) == n == len(proofs):
+            raise ValueError(f"{n} blobs, {len(commitments)} commitments and {len(proofs)} proofs")
+        for b in blobs:
+            self._check_len("blob", b, self.BYTES_PER_BLOB)
+        for c in commitments:
+            self._check_len("commitment", c, 48)
+        for p in proofs:
+            self._check_len("proof", p, 48)
+        self._check_len("secure_random_bytes", secure_random_bytes, 32)
+        rc = _lib.load().ctt_b200_eth_kzg_verify_blob_kzg_proof_batch(self._h, _buf(b"".join(blobs) or b"\0"),
+                                                                      _buf(b"".join(commitments) or b"\0"),
+                                                                      _buf(b"".join(proofs) or b"\0"), n, _buf(bytes(secure_random_bytes)))
+        return self._verify_status(rc)
+
     @staticmethod
     def last_verify_timing() -> dict:
-        """Host checks + challenge, device decode, scalar kernels, bank MSM (CUDA events) and host pairing time (ms) of the calling
-        thread's last verify_cell_kzg_proof_batch."""
+        """Host checks + challenges, device decode, scalar kernels, bank MSM (CUDA events) and host pairing time (ms) of the calling
+        thread's last verification of either family (cells or blobs)."""
         v = [ctypes.c_float(0) for _ in range(5)]
         _lib.load().ctt_b200_eth_kzg_last_verify_timing(*[ctypes.byref(x) for x in v])
         return dict(zip(("ms_host", "ms_decode", "ms_fr", "ms_msm", "ms_pairing"), (x.value for x in v)))

@@ -6,9 +6,11 @@ bank MSM with its engine phases, EC FFTs). The recovery leg: recover_cells_and_k
 blob, as n single calls against one batched call, and the same split. The verify leg: verify_cell_kzg_proof_batch over n cells of 72
 random blobs (n = 128, 6 x 128, 21 x 128, 72 x 128 shuffled; one column of 72; 8 columns of 72), with the Fiat-Shamir challenge and with
 caller-supplied random bytes: the median per call and its split (host checks + challenge, device decode, scalar kernels, bank MSM,
-host pairing). Prints one JSON line.
+host pairing). The verify4844 leg: verify_blob_kzg_proof_batch over n seeded random blobs with their device-computed commitments and
+proofs, with the Fiat-Shamir r and with caller-supplied random bytes, the same split, and the single entries verify_blob_kzg_proof and
+verify_kzg_proof. Prints one JSON line.
 python tools/bench_kzg.py [--reps R] [--sizes 1,6,9,32,128] [--das-sizes 1,6,21,72] [--rec-sizes 1,6,21,72] [--verify-sizes 1,6,21,72]
-                          [--only verify]"""
+                          [--verify4844-sizes 1,6,72,1024] [--only verify|verify4844]"""
 import argparse
 import json
 import os
@@ -118,6 +120,34 @@ def verify(ctx, sizes, reps):
     return r
 
 
+def verify4844(ctx, sizes, reps):
+    """verify_blob_kzg_proof_batch over n blobs (both r paths) and the single entries; needs only the G2 setup."""
+    ctx.load_g2_setup(np.load(os.path.join(ROOT, "tests", "golden", "peerdas_verify_kat.npz"))["srs_monomial_g2_compressed"].tobytes())
+    blobs = random_blobs(max(sizes), 4845)
+    cms = ctx.blobs_to_kzg_commitments(blobs)
+    proofs = ctx.compute_blob_kzg_proofs(blobs, cms)
+    r = {}
+
+    def split(fn):
+        assert fn()
+        fn()
+        s = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            fn()
+            s.append({"wall_ms": (time.perf_counter() - t0) * 1e3, **ctx.last_verify_timing()})
+        return {k: round(statistics.median(x[k] for x in s), 3) for k in s[0]}
+    for n in sizes:
+        a = (blobs[:n], cms[:n], proofs[:n])
+        for path, rb in (("fs", bytes(32)), ("rand", bytes(range(1, 33)))):
+            r[f"batch_n{n}_{path}_ms"] = split(lambda: ctx.verify_blob_kzg_proof_batch(*a, secure_random_bytes=rb))
+    r["blob_proof_single_ms"] = split(lambda: ctx.verify_blob_kzg_proof(blobs[0], cms[0], proofs[0]))
+    z = (4844).to_bytes(32, "big")
+    proof, y = ctx.compute_kzg_proof(blobs[0], z)
+    r["kzg_proof_single_ms"] = split(lambda: ctx.verify_kzg_proof(cms[0], z, y, proof))
+    return r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
@@ -125,12 +155,18 @@ def main():
     ap.add_argument("--das-sizes", default="1,6,21,72")
     ap.add_argument("--rec-sizes", default="1,6,21,72")
     ap.add_argument("--verify-sizes", default="1,6,21,72")
-    ap.add_argument("--only", default="", help="'verify': only the verify leg (after load_peerdas)")
+    ap.add_argument("--verify4844-sizes", default="1,6,72,1024")
+    ap.add_argument("--only", default="", help="'verify': only the verify leg (after load_peerdas); 'verify4844': only the verify4844 leg")
     a = ap.parse_args()
     sizes = [int(s) for s in a.sizes.split(",")]
     srs = np.load(os.path.join(ROOT, "tests", "golden", "kzg_commit_kat.npz"))["srs_lagrange_brp_compressed"].tobytes()
     ctx = M.EthKzgContext(srs, compressed=True)
     vsizes = [int(s) for s in a.verify_sizes.split(",")]
+    v4sizes = [int(s) for s in a.verify4844_sizes.split(",")]
+    if a.only == "verify4844":
+        print(json.dumps({"gpu": bench.gpu_identity(0), "reps": a.reps, "verify4844": verify4844(ctx, v4sizes, a.reps)}), flush=True)
+        ctx.delete()
+        return
     if a.only == "verify":
         ctx.load_peerdas(np.load(os.path.join(ROOT, "tests", "golden", "peerdas_kat.npz"))["srs_monomial_compressed"].tobytes())
         print(json.dumps({"gpu": bench.gpu_identity(0), "reps": a.reps, "verify": verify(ctx, vsizes, a.reps)}), flush=True)
@@ -161,6 +197,7 @@ def main():
     out["peerdas"] = peerdas(ctx, [int(s) for s in a.das_sizes.split(",")], a.reps)
     out["recovery"] = recovery(ctx, [int(s) for s in a.rec_sizes.split(",")], a.reps)
     out["verify"] = verify(ctx, vsizes, a.reps)
+    out["verify4844"] = verify4844(ctx, v4sizes, a.reps)
     ctx.delete()
     print(json.dumps(out), flush=True)
 

@@ -4,6 +4,8 @@
 //   challenge <blob> <commit>    -> the Fiat-Shamir challenge of compute_blob_kzg_proof, 32 bytes big-endian (hex)
 //   commitment <hex48>           -> the cttEthKzg status of bytes_to_kzg_commitment
 //   roots                        -> the 4096 brp roots of unity, canonical, 32 bytes big-endian (hex), one per line
+//   blinding <bytes32> <n> <z_1> .. <z_n>  -> the r of verify_blob_kzg_proof_batch for those caller bytes and opening challenges (each
+//                                   32 bytes big-endian, canonical): "<1 if the caller's bytes were used, else 0> <r, 32 bytes big-endian>"
 #include <cstdio>
 #include <iostream>
 #include <string>
@@ -56,6 +58,23 @@ int main() {
         limbs_to_be32(out, c);
         std::cout << hex(out, 32) << "\n";
       }
+    } else if (cmd == "blinding") {
+      std::string rb;
+      size_t n = 0;
+      std::cin >> rb >> n;
+      const std::vector<uint8_t> rnd = unhex(rb);
+      std::vector<Fr> zm(n);
+      for (size_t i = 0; i < n; i++) {
+        std::string a; std::cin >> a;
+        uint64_t z[4];
+        be32_to_limbs(z, unhex(a).data());
+        zm[i] = fr_to_mont(z);
+      }
+      uint64_t r[4];
+      const bool caller = blob_batch_blinding(r, rnd.data(), zm.data(), n);
+      uint8_t out[32];
+      limbs_to_be32(out, r);
+      std::cout << (caller ? 1 : 0) << " " << hex(out, 32) << "\n";
     } else {
       std::cout << "unknown\n";
     }

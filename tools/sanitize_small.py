@@ -1,5 +1,6 @@
 #!/usr/bin/env python3
-"""Small MSMs on every curve, a 2-blob PeerDAS recovery and a 40-cell batch verification, meant to run under compute-sanitizer (memcheck / racecheck):
+"""Small MSMs on every curve, a 2-blob PeerDAS recovery, a 40-cell batch verification and a 3-blob
+EIP-4844 batch verification, meant to run under compute-sanitizer (memcheck / racecheck):
    compute-sanitizer --tool racecheck python tools/sanitize_small.py"""
 import os, random, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -38,4 +39,9 @@ picks = [(r.randrange(2), r.randrange(128)) for _ in range(40)]
 ok = ctx.verify_cell_kzg_proof_batch([cms[b] for b, _ in picks], [c for _, c in picks], [full[b][0][c] for b, c in picks],
                                      [full[b][1][c] for b, c in picks])
 print("verify 40 cells", "OK" if ok else "MISMATCH", flush=True)
+# a 3-blob verify_blob_kzg_proof_batch (decode, parse, evaluation and scalar kernels, the bank MSM)
+b3 = [bytes(commit["blobs"][j]) for j in (1, 2, 3)]
+c3 = ctx.blobs_to_kzg_commitments(b3)
+ok = ctx.verify_blob_kzg_proof_batch(b3, c3, ctx.compute_blob_kzg_proofs(b3, c3), secure_random_bytes=bytes(range(32)))
+print("verify 3 blobs", "OK" if ok else "MISMATCH", flush=True)
 ctx.delete()
