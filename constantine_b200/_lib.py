@@ -142,6 +142,23 @@ def load():
     lib.ctt_b200_eth_kzg_verify_blob_kzg_proof_batch.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_kzg_last_verify_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 5
     lib.ctt_b200_eth_kzg_last_verify_timing.restype = None
+    ub = ctypes.c_uint8
+    lib.ctt_eth_bls_batch_verify.argtypes = [vp, vp, vp, sz, vp]
+    lib.ctt_eth_bls_batch_verify.restype = ub
+    lib.ctt_eth_bls_batch_verify_parallel.argtypes = [vp, vp, vp, vp, sz, vp]
+    lib.ctt_eth_bls_batch_verify_parallel.restype = ub
+    lib.ctt_eth_bls_aggregate_verify.argtypes = [vp, vp, sz, vp]
+    lib.ctt_eth_bls_aggregate_verify.restype = ub
+    lib.ctt_b200_eth_bls_deserialize_pubkey_compressed.argtypes = [vp, vp]
+    lib.ctt_b200_eth_bls_deserialize_pubkey_compressed.restype = ci
+    lib.ctt_b200_eth_bls_deserialize_signature_compressed.argtypes = [vp, vp]
+    lib.ctt_b200_eth_bls_deserialize_signature_compressed.restype = ci
+    lib.ctt_b200_eth_bls_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 6
+    lib.ctt_b200_eth_bls_last_timing.restype = None
+    lib.ctt_b200_test_hash_to_g2.argtypes = [vp, sz, vp, sz, vp]
+    lib.ctt_b200_test_hash_to_g2.restype = ci
+    lib.ctt_b200_test_pairing.argtypes = [vp, vp, sz, vp]
+    lib.ctt_b200_test_pairing.restype = ci
     lib.ctt_threadpool_new.argtypes = [ci]
     lib.ctt_threadpool_new.restype = vp
     lib.ctt_threadpool_shutdown.argtypes = [vp]

@@ -113,20 +113,6 @@ static void batch_affine(const HP* p, size_t count, Fp* xy) {
 struct Timing { float ms_host = 0, ms_quotient = 0; };
 static Timing& last_timing() { static thread_local Timing t; return t; }
 
-// fn(j) for j < n on up to hardware_concurrency host threads (the per-blob checks and challenges of a batch: SHA-256 over 128 KiB and
-// a subgroup check each, ~0.8 ms of host time per blob that would otherwise run one after the other)
-template <class Fn>
-static void parallel_for(size_t n, Fn fn) {
-  size_t t = std::thread::hardware_concurrency();
-  if (t > n) t = n;
-  if (t > 32) t = 32;
-  if (t <= 1) { for (size_t j = 0; j < n; j++) fn(j); return; }
-  std::vector<std::thread> th;
-  for (size_t w = 0; w < t; w++)
-    th.emplace_back([&, w] { for (size_t j = w; j < n; j += t) fn(j); });
-  for (auto& x : th) x.join();
-}
-
 static double ms_since(std::chrono::steady_clock::time_point t0) {
   return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
@@ -248,11 +234,6 @@ static G1Aff xyzz_affine(const HP& p) {
 }
 
 // ---- EIP-4844 verification ---------------------------------------------------------------------------------------------------
-// The G1 generator, 48-byte compressed: the last point of the blob entries' MSM point set, and [y]G1 of verify_kzg_proof
-static const uint8_t G1_GENERATOR[48] = {
-    0x97, 0xf1, 0xd3, 0xa7, 0x31, 0x97, 0xd7, 0x94, 0x26, 0x95, 0x63, 0x8c, 0x4f, 0xa9, 0xac, 0x0f, 0xc3, 0x68, 0x8c, 0x4f, 0x97, 0x74, 0xb9, 0x05,
-    0xa1, 0x4e, 0x3a, 0x3f, 0x17, 0x1b, 0xac, 0x58, 0x6c, 0x55, 0xe8, 0x3f, 0xf9, 0x7a, 0x1a, 0xef, 0xfb, 0x3a, 0xf0, 0x0a, 0xdb, 0x22, 0xc6, 0xbb};
-
 static HP affine_xyzz(const Fp& x, const Fp& y) {
   if (x.is_zero() && y.is_zero()) return HP::inf();
   HP p; p.x = x; p.y = y; p.zz = Fp::one(); p.zzz = Fp::one();

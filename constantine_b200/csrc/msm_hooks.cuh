@@ -95,12 +95,14 @@ int run_sum_partials(int out_kind, void* r, const void* partials, size_t count) 
   return 0;
 }
 
-// out[i] = [k[i]] * base, normalised to affine -- synthetic-input generator (bench / tests) and naive scalar-mul hook.
+// out[i] = [k[i]] * base, normalised to affine -- synthetic-input generator (bench / tests) and naive scalar-mul hook. With
+// per_item_base, item i takes base point i (the blinding [r_i]PK_i of the BLS batch verification, eth_bls.cu).
 template <class T>
-__global__ void __launch_bounds__(128) k_scalar_mul_u64(const uint32_t* base, const unsigned long long* k, size_t count, uint32_t* out) {
+__global__ void __launch_bounds__(128) k_scalar_mul_u64(const uint32_t* base, const unsigned long long* k, size_t count, uint32_t* out,
+                                                        bool per_item_base = false) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
-  Aff<T> B = load_affine<T>(base, 0);
+  Aff<T> B = load_affine<T>(base, per_item_base ? (uint32_t)i : 0u);
   unsigned long long s = k[i];
   Xyzz<T> acc = Xyzz<T>::inf();
 #pragma unroll 1

@@ -292,6 +292,92 @@ def eth_evm_bls12381_g2msm(inputs: bytes, out_len: int = 256):
     return EVM_STATUS[st], r.raw
 
 
+class CtSpan(ctypes.Structure):
+    """ctt_span: {byte* data; size_t len} (reference include/constantine/protocols/ethereum_bls_signatures.h:64)."""
+    _fields_ = [("data", ctypes.c_void_p), ("len", ctypes.c_size_t)]
+
+
+ETH_BLS_PUBKEY_BYTES, ETH_BLS_SIGNATURE_BYTES = 96, 192   # affine Montgomery structs (ctt_eth_bls_pubkey / ctt_eth_bls_signature)
+
+
+def eth_bls_deserialize_pubkey(b48: bytes) -> bytes:
+    """48-byte compressed public key -> the 96-byte ctt_eth_bls_pubkey struct (curve and subgroup checked). Raises
+    ValueError(status) with the reference's ctt_codec_ecc_status when it is not Success (5 = PointAtInfinity included)."""
+    if len(b48) != 48:
+        raise ValueError("a compressed public key is 48 bytes, got %d" % len(b48))
+    out = ctypes.create_string_buffer(ETH_BLS_PUBKEY_BYTES)
+    st = _lib.load().ctt_b200_eth_bls_deserialize_pubkey_compressed(out, _buf(bytes(b48)))
+    if st != 0:
+        raise ValueError(st)
+    return out.raw
+
+
+def eth_bls_deserialize_signature(b96: bytes) -> bytes:
+    """96-byte compressed signature -> the 192-byte ctt_eth_bls_signature struct, as eth_bls_deserialize_pubkey."""
+    if len(b96) != 96:
+        raise ValueError("a compressed signature is 96 bytes, got %d" % len(b96))
+    out = ctypes.create_string_buffer(ETH_BLS_SIGNATURE_BYTES)
+    st = _lib.load().ctt_b200_eth_bls_deserialize_signature_compressed(out, _buf(bytes(b96)))
+    if st != 0:
+        raise ValueError(st)
+    return out.raw
+
+
+def _eth_bls_items(items, size, what):
+    for x in items:
+        if len(x) != size:
+            raise ValueError("every %s struct is %d bytes, got %d" % (what, size, len(x)))
+    return b"".join(bytes(x) for x in items)
+
+
+def _eth_bls_spans(messages):
+    keep = [ctypes.create_string_buffer(bytes(m), max(1, len(m))) for m in messages]
+    spans = (CtSpan * max(1, len(messages)))()
+    for i, (m, b) in enumerate(zip(messages, keep)):
+        spans[i].data = ctypes.cast(b, ctypes.c_void_p)
+        spans[i].len = len(m)
+    return spans, keep
+
+
+def eth_bls_batch_verify(pubkeys, messages, signatures, secure_random_bytes: bytes) -> bool:
+    """ctt_eth_bls_batch_verify over lists of public key structs (96 bytes), messages and signature structs (192 bytes). True on
+    Success; False on VerificationFailure, ZeroLengthAggregation (empty lists) or PointAtInfinity. Lists of unequal length or
+    items of the wrong size raise ValueError before the call."""
+    if not (len(pubkeys) == len(messages) == len(signatures)):
+        raise ValueError("pubkeys, messages and signatures differ in length: %d, %d, %d" % (len(pubkeys), len(messages), len(signatures)))
+    if len(secure_random_bytes) != 32:
+        raise ValueError("secure_random_bytes is 32 bytes, got %d" % len(secure_random_bytes))
+    pk = _eth_bls_items(pubkeys, ETH_BLS_PUBKEY_BYTES, "public key")
+    sg = _eth_bls_items(signatures, ETH_BLS_SIGNATURE_BYTES, "signature")
+    spans, _keep = _eth_bls_spans(messages)
+    st = _lib.load().ctt_eth_bls_batch_verify(_buf(pk or b"\0"), spans, _buf(sg or b"\0"), len(pubkeys), _buf(bytes(secure_random_bytes)))
+    if st not in (0, 1, 3, 4):
+        raise ValueError(st)
+    return st == 0
+
+
+def eth_bls_aggregate_verify(pubkeys, messages, aggregate_sig: bytes) -> bool:
+    """ctt_eth_bls_aggregate_verify: the public keys (96-byte structs) each signed its message, and aggregate_sig (a 192-byte struct)
+    is the sum of their signatures. Return values and errors as eth_bls_batch_verify."""
+    if len(pubkeys) != len(messages):
+        raise ValueError("pubkeys and messages differ in length: %d, %d" % (len(pubkeys), len(messages)))
+    pk = _eth_bls_items(pubkeys, ETH_BLS_PUBKEY_BYTES, "public key")
+    sg = _eth_bls_items([aggregate_sig], ETH_BLS_SIGNATURE_BYTES, "signature")
+    spans, _keep = _eth_bls_spans(messages)
+    st = _lib.load().ctt_eth_bls_aggregate_verify(_buf(pk or b"\0"), spans, len(pubkeys), _buf(sg))
+    if st not in (0, 1, 3, 4):
+        raise ValueError(st)
+    return st == 0
+
+
+def eth_bls_last_timing() -> dict:
+    """Host checks with expand_message_xmd and the blinding chain, device hash to G2, blinding, Miller loops, final exponentiation
+    (CUDA events) and the G2 MSM (ms) of the calling thread's last BLS verification."""
+    v = [ctypes.c_float(0) for _ in range(6)]
+    _lib.load().ctt_b200_eth_bls_last_timing(*[ctypes.byref(x) for x in v])
+    return dict(zip(("ms_host", "ms_hash", "ms_blind", "ms_msm", "ms_miller", "ms_final"), (x.value for x in v)))
+
+
 class EthKzgContext:
     """EIP-4844 commitment context on the resident SRS, the role of the reference's EthereumKZGContext for
     blob_to_kzg_commitment[_parallel] (reference constantine/ethereum_eip4844_kzg_parallel.nim:125-159)."""

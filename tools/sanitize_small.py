@@ -45,3 +45,19 @@ c3 = ctx.blobs_to_kzg_commitments(b3)
 ok = ctx.verify_blob_kzg_proof_batch(b3, c3, ctx.compute_blob_kzg_proofs(b3, c3), secure_random_bytes=bytes(range(32)))
 print("verify 3 blobs", "OK" if ok else "MISMATCH", flush=True)
 ctx.delete()
+# a 3-signature BLS batch_verify (hash to G2, blinding, Miller loops, tree product, final exponentiation, the G2 MSM)
+import ctypes
+import bls_exact as B
+from constantine_b200 import _lib
+lib = _lib.load()
+msgs = [b"sanitize-%d" % k for k in range(3)]
+sks = [r.getrandbits(63) | 1 for _ in range(3)]
+pks, sigs = [], []
+for m, k in zip(msgs, sks):
+    out, h = ctypes.create_string_buffer(192), ctypes.create_string_buffer(192)
+    lib.ctt_b200_scalar_mul_u64(0, B.g1_struct(B.g1_generator()), (ctypes.c_uint64 * 1)(k), 1, out)
+    pks.append(out.raw[:96])
+    lib.ctt_b200_test_hash_to_g2(m, len(m), B.POP_DST, len(B.POP_DST), h)
+    lib.ctt_b200_scalar_mul_u64(4, h, (ctypes.c_uint64 * 1)(k), 1, out)
+    sigs.append(out.raw)
+print("bls batch 3", "OK" if M.eth_bls_batch_verify(pks, msgs, sigs, bytes(range(32))) else "MISMATCH", flush=True)
