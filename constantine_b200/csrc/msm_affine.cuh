@@ -488,4 +488,298 @@ k_affine_pairs(const void* __restrict__ plan, const uint32_t* __restrict__ total
   }
 }
 
+// ------------------------------------------------------------------------------------------------ warp-specialised pair kernel
+// Same slots, same per-thread batches, same arithmetic as k_affine_pairs (so the same results), but the operand gathers are moved
+// out of the threads that multiply. A block is AFF_WS_CONSUMERS consumer warps plus ONE producer warp. Consumer warp w owns the
+// slots k_affine_pairs would give a warp (a contiguous range of 32 M slots, lane l takes l, l + 32, ...). For every consumer warp,
+// in the order that warp consumes them, the producer reads the plan entry and issues cp.async copies of the operands into a ring of
+// stages in shared memory (pass 1: x1, x2; pass 2: P1, P2 and the slot's prefix product), then signals the stage's `full` mbarrier
+// (cp.async.mbarrier.arrive.noinc: the arrival lands when the copies have). A consumer waits on `full`, reads the stage into
+// registers, frees it on `empty` and multiplies; the random point gathers are in flight while it computes, and none of them holds a
+// consumer register. Pass-1 stages (2 elements per slot) are smaller than pass-2 stages (5 elements), so the same ring holds more of
+// them. One producer warp costs 1 / (AFF_WS_CONSUMERS + 1) of the register file, so no setmaxnreg rebalancing is needed: at one
+// block per SM every thread may use the registers the unrolled multipliers want.
+// Only for coordinates of up to 12 words: a pass-2 stage of Fp2 points (24 words) would need 15 KiB per consumer warp.
+#ifndef B200_AFF_WS_CONSUMERS
+#define B200_AFF_WS_CONSUMERS 8
+#endif
+#ifndef B200_AFF_WS_STAGES
+#define B200_AFF_WS_STAGES 2
+#endif
+constexpr int AFF_WS_CONSUMERS = B200_AFF_WS_CONSUMERS;
+constexpr int AFF_WS_THREADS = 32 * (AFF_WS_CONSUMERS + 1);
+
+template <class T>
+struct AffRing {
+  static constexpr bool USED = T::WORDS <= 12;
+  static constexpr int V = T::WORDS / 4;                // 16-byte vectors per field element
+  static constexpr int S2 = B200_AFF_WS_STAGES;         // pass-2 stages per consumer warp: P1, P2, prefix product
+  static constexpr int ROWS = S2 * 5 * V;               // rows of 32 lanes x 16 B in a consumer warp's ring
+  static constexpr int S1 = ROWS / (2 * V);             // pass-1 stages (x1, x2) in the same bytes
+  static constexpr size_t BYTES = (size_t)AFF_WS_CONSUMERS * ROWS * 32 * 16;
+};
+
+B200_DEV uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+B200_DEV void mbar_init(uint64_t* b, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(b)), "r"(count) : "memory"); }
+B200_DEV void mbar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(b)) : "memory"); }
+B200_DEV void mbar_wait(uint64_t* b, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred P1;\n"
+      "WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
+      "@!P1 bra WAIT;\n\t}" ::"r"(smem_addr(b)),
+      "r"(parity)
+      : "memory");
+}
+// arrival on b once every cp.async this thread has issued so far has landed (counted in b's expected arrivals)
+B200_DEV void cp_async_arrive(uint64_t* b) { asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_addr(b)) : "memory"); }
+B200_DEV void cp_async16(void* s, const void* g) { asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr(s)), "l"(g) : "memory"); }
+
+// ring rows are [row][lane] uint4: every access of a warp is one conflict-free 512-byte row
+template <class T>
+B200_DEV void ring_fetch(uint4* ring, int row, unsigned lane, const uint32_t* g) {
+#pragma unroll
+  for (int k = 0; k < T::WORDS / 4; k++) cp_async16(ring + (row + k) * 32 + lane, g + 4 * k);
+}
+template <class T>
+B200_DEV T ring_load(const uint4* ring, int row, unsigned lane) {
+  T v;
+#pragma unroll
+  for (int k = 0; k < T::WORDS / 4; k++) {
+    const uint4 w = ring[(row + k) * 32 + lane];
+    v.set_word(4 * k + 0, w.x); v.set_word(4 * k + 1, w.y); v.set_word(4 * k + 2, w.z); v.set_word(4 * k + 3, w.w);
+  }
+  return v;
+}
+
+template <class T, bool FIRST>
+__global__ void __launch_bounds__(AFF_WS_THREADS, 1)
+k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ total_ptr, const uint32_t* src, uint32_t* dst, uint4* scratch,
+                  const uint32_t* __restrict__ perm = nullptr, const uint32_t* __restrict__ range = nullptr) {
+  using RG = AffRing<T>;
+  constexpr int V = RG::V, NC = AFF_WS_CONSUMERS, S1 = RG::S1, S2 = RG::S2;
+  extern __shared__ __align__(16) unsigned char aff_ring_raw[];
+  __shared__ uint64_t full1[NC][S1], empty1[NC][S1], full2[NC][S2], empty2[NC][S2], drained[NC];
+  __shared__ uint32_t s_task[NC][S1][3][32];          // (a, b, output slot) of each lane's slot in a stage
+  const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) {
+    for (int w = 0; w < NC; w++) {
+      for (int s = 0; s < S1; s++) { mbar_init(&full1[w][s], 64); mbar_init(&empty1[w][s], 32); }   // full: 32 copy + 32 task arrivals
+      for (int s = 0; s < S2; s++) { mbar_init(&full2[w][s], 64); mbar_init(&empty2[w][s], 32); }
+      mbar_init(&drained[w], 32);
+    }
+  }
+  __syncthreads();
+  // slots as in k_affine_pairs, over the consumer threads only
+  const size_t threads = (size_t)gridDim.x * NC * 32;
+  const uint32_t range_begin = range ? range[0] : 0u;
+  const uint32_t total = range ? range[1] - range[0] : *total_ptr;
+  if (perm) perm += range_begin;
+  const uint32_t M = (uint32_t)(((size_t)total + threads - 1) / threads);
+  auto count_of = [&](size_t tid) -> uint32_t {      // slots of consumer thread tid: warp_base + lane + 32 j, j < count
+    const size_t first = (tid & ~(size_t)31) * M + (tid & 31u);
+    if (first >= total) return 0u;
+    const uint32_t c = (uint32_t)(((size_t)total - first + 31) / 32);
+    return c < M ? c : M;
+  };
+  auto slot_at = [&](size_t tid, uint32_t j) -> size_t {
+    const size_t t = (tid & ~(size_t)31) * M + (tid & 31u) + 32u * (size_t)j;
+    return perm ? (size_t)perm[t] : t;
+  };
+  uint4* const ring_base = reinterpret_cast<uint4*>(aff_ring_raw);
+
+  if (warp == NC) {
+    // ================= producer: lane l fetches for lane l of every consumer warp
+    uint32_t n[NC], cnt[NC];
+#pragma unroll
+    for (int w = 0; w < NC; w++) {
+      const size_t tid = ((size_t)blockIdx.x * NC + w) * 32 + lane;
+      n[w] = count_of(tid - lane);                   // iterations of warp w (lane 0 has the most slots)
+      cnt[w] = count_of(tid);
+    }
+    auto tid_of = [&](int w) { return ((size_t)blockIdx.x * NC + w) * 32 + lane; };
+    auto src_of = [&](uint32_t ref) { return src + (size_t)(FIRST ? (ref & 0x7FFFFFFFu) : ref) * (2 * T::WORDS); };
+    // the plan entries of the next round are loaded while this round's copies are issued
+    uint32_t ta[NC], tb[NC], tp[NC];
+    auto fetch_task = [&](int w, uint32_t j) {
+      const size_t p = slot_at(tid_of(w), j);
+      const PairTask t = load_task<FIRST>(plan, p);
+      ta[w] = t.a; tb[w] = t.b; tp[w] = (uint32_t)p;
+    };
+    // ---- pass 1: x1, x2
+#pragma unroll
+    for (int w = 0; w < NC; w++) if (cnt[w]) fetch_task(w, 0);
+#pragma unroll 1
+    for (uint32_t j = 0; j < n[0]; j++) {
+      uint32_t ca[NC], cb[NC];
+#pragma unroll
+      for (int w = 0; w < NC; w++) { ca[w] = ta[w]; cb[w] = tb[w]; }
+#pragma unroll
+      for (int w = 0; w < NC; w++) if (j + 1 < cnt[w]) fetch_task(w, j + 1);
+#pragma unroll
+      for (int w = 0; w < NC; w++) {
+        if (j >= n[w]) continue;
+        const int s = (int)(j % S1);
+        mbar_wait(&empty1[w][s], ((j / S1) & 1u) ^ 1u);
+        uint4* ring = ring_base + (size_t)w * RG::ROWS * 32;
+        if (j < cnt[w]) {
+          s_task[w][s][0][lane] = ca[w];
+          s_task[w][s][1][lane] = cb[w];
+          ring_fetch<T>(ring, s * 2 * V, lane, src_of(ca[w]));
+          if (cb[w] != AFF_NONE) ring_fetch<T>(ring, s * 2 * V + V, lane, src_of(cb[w]));
+        }
+        cp_async_arrive(&full1[w][s]);
+        mbar_arrive(&full1[w][s]);
+      }
+    }
+    // ---- pass 2, last slot first: P1, P2, prefix product of the slot before
+#pragma unroll
+    for (int w = 0; w < NC; w++) if (n[w] && n[w] - 1 < cnt[w]) fetch_task(w, n[w] - 1);
+#pragma unroll 1
+    for (uint32_t jj = 0; jj < n[0]; jj++) {
+      uint32_t ca[NC], cb[NC], cp[NC];
+#pragma unroll
+      for (int w = 0; w < NC; w++) { ca[w] = ta[w]; cb[w] = tb[w]; cp[w] = tp[w]; }
+#pragma unroll
+      for (int w = 0; w < NC; w++) if (jj + 1 < n[w] && n[w] - 2 - jj < cnt[w]) fetch_task(w, n[w] - 2 - jj);
+#pragma unroll
+      for (int w = 0; w < NC; w++) {
+        if (jj >= n[w]) continue;
+        if (jj == 0) mbar_wait(&drained[w], 0);      // warp w has read its last pass-1 stage and stored all its prefix products
+        const uint32_t j = n[w] - 1 - jj;
+        const int s = (int)(jj % S2);
+        mbar_wait(&empty2[w][s], ((jj / S2) & 1u) ^ 1u);
+        uint4* ring = ring_base + (size_t)w * RG::ROWS * 32;
+        if (j < cnt[w]) {
+          s_task[w][s][0][lane] = ca[w];
+          s_task[w][s][1][lane] = cb[w];
+          s_task[w][s][2][lane] = cp[w];
+          const int row = s * 5 * V;
+          ring_fetch<T>(ring, row, lane, src_of(ca[w]));
+          ring_fetch<T>(ring, row + V, lane, src_of(ca[w]) + T::WORDS);
+          if (cb[w] != AFF_NONE) {
+            ring_fetch<T>(ring, row + 2 * V, lane, src_of(cb[w]));
+            ring_fetch<T>(ring, row + 3 * V, lane, src_of(cb[w]) + T::WORDS);
+          }
+          if (j > 0) {
+#pragma unroll
+            for (int k = 0; k < V; k++)
+              cp_async16(ring + (row + 4 * V + k) * 32 + lane, scratch + ((size_t)(j - 1) * V + k) * threads + tid_of(w));
+          }
+        }
+        cp_async_arrive(&full2[w][s]);
+        mbar_arrive(&full2[w][s]);
+      }
+    }
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    return;
+  }
+
+  // ================= consumers
+  const size_t tid = ((size_t)blockIdx.x * NC + warp) * 32 + lane;
+  const uint32_t n = count_of(tid - lane), cnt = count_of(tid);
+  if (n == 0) return;
+  const uint4* ring = ring_base + (size_t)warp * RG::ROWS * 32;
+  // ---- pass 1: running product of the denominators; prefix products to the scratch
+  T run = T::one();
+#pragma unroll 1
+  for (uint32_t j = 0; j < n; j++) {
+    const int s = (int)(j % S1);
+    mbar_wait(&full1[warp][s], (j / S1) & 1u);
+    const uint32_t a = s_task[warp][s][0][lane], b = s_task[warp][s][1][lane];
+    const T x1 = ring_load<T>(ring, s * 2 * V, lane), x2 = ring_load<T>(ring, s * 2 * V + V, lane);
+    mbar_arrive(&empty1[warp][s]);
+    if (j >= cnt) continue;
+    const bool single = b == AFF_NONE;
+    T den = x2 - x1;
+    bool contributes = !single;
+    if (!single && (den.is_zero() || x1.is_zero() || x2.is_zero())) {
+      // rare: equal abscissae (doubling or cancellation) or a possible infinity operand -- needs the ordinates
+      bool z1, z2;
+      const T y1 = load_y<T, FIRST>(src, a, z1), y2 = load_y<T, FIRST>(src, b, z2);
+      const int kind = classify_pair(false, x1, y1, z1 && x1.is_zero(), x2, y2, z2 && x2.is_zero(), den);
+      contributes = kind >= PAIR_ADD;
+    }
+    if (contributes) run = run.mul_u(den);
+    scratch_store(scratch, threads, tid, j, run);
+  }
+  mbar_arrive(&drained[warp]);      // release: the producer's pass-2 copies of the prefix products come after these stores
+  // ---- the shared inversion of this thread's batch
+  T inv = fe_inverse(run);
+  // ---- pass 2: unwind, last slot first
+#pragma unroll 1
+  for (uint32_t jj = 0; jj < n; jj++) {
+    const uint32_t j = n - 1 - jj;
+    const int s = (int)(jj % S2);
+    mbar_wait(&full2[warp][s], (jj / S2) & 1u);
+    const int row = s * 5 * V;
+    const uint32_t a = s_task[warp][s][0][lane], b = s_task[warp][s][1][lane], p = s_task[warp][s][2][lane];
+    const bool single = b == AFF_NONE;
+    Aff<T> P1, P2;
+    P1.x = ring_load<T>(ring, row, lane);
+    P1.y = ring_load<T>(ring, row + V, lane);
+    P2.x = single ? T::zero() : ring_load<T>(ring, row + 2 * V, lane);
+    P2.y = single ? T::zero() : ring_load<T>(ring, row + 3 * V, lane);
+    const T pre = ring_load<T>(ring, row + 4 * V, lane);
+    mbar_arrive(&empty2[warp][s]);
+    if (j >= cnt) continue;
+    const bool z1 = P1.y.is_zero(), z2 = P2.y.is_zero();
+    if constexpr (FIRST) {
+      P1.y.cneg((a >> 31) != 0);
+      if (!single) P2.y.cneg((b >> 31) != 0);
+    }
+    T den;
+    const int kind = classify_pair(single, P1.x, P1.y, z1 && P1.x.is_zero(), P2.x, P2.y, z2 && P2.x.is_zero(), den);
+    Aff<T> R;
+    if (kind < PAIR_ADD) {
+      if (kind == PAIR_COPY1) R = P1;
+      else if (kind == PAIR_COPY2) R = P2;
+      else { R.x = T::zero(); R.y = T::zero(); }
+    } else {
+      T inv_den = inv;
+      if (j > 0) inv_den = inv.mul_u(pre);
+      inv = inv.mul_u(den);
+      T num;
+      if (kind == PAIR_ADD) num = P2.y - P1.y;
+      else { const T xx = P1.x.sqr(); num = xx.dbl() + xx; }     // 3 x^2 (a = 0); rare: rolled multiplier
+      const T lam = num.mul_u(inv_den);
+      R.x = lam.sqr_u() - P1.x - P2.x;
+      R.y = lam.mul_u(P1.x - R.x) - P1.y;
+    }
+    store_affine(dst, p, R);
+  }
+}
+
+// Pair kernel of a level: the warp-specialised one where its ring fits in shared memory, k_affine_pairs otherwise.
+template <class T>
+constexpr int affine_pairs_slot_threads() { return AffRing<T>::USED ? 32 * AFF_WS_CONSUMERS : B200_AFF_THREADS; }   // threads per block that own slots
+
+// resident blocks per SM of the pair kernel (also raises the dynamic shared-memory limit of the warp-specialised kernel)
+template <class T>
+cudaError_t affine_pairs_blocks_per_sm(int* bps) {
+  int b1 = 0, b2 = 0;
+  cudaError_t e;
+  if constexpr (AffRing<T>::USED) {
+    constexpr int bytes = (int)AffRing<T>::BYTES;
+    if ((e = cudaFuncSetAttribute(k_affine_pairs_ws<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_affine_pairs_ws<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)) != cudaSuccess) return e;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, k_affine_pairs_ws<T, true>, AFF_WS_THREADS, bytes)) != cudaSuccess) return e;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, k_affine_pairs_ws<T, false>, AFF_WS_THREADS, bytes)) != cudaSuccess) return e;
+  } else {
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, k_affine_pairs<T, true>, B200_AFF_THREADS, 0)) != cudaSuccess) return e;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, k_affine_pairs<T, false>, B200_AFF_THREADS, 0)) != cudaSuccess) return e;
+  }
+  *bps = b2 < b1 ? b2 : b1;
+  return cudaSuccess;
+}
+
+template <class T, bool FIRST>
+void launch_affine_pairs(unsigned grid, cudaStream_t s, const void* plan, const uint32_t* total_ptr, const uint32_t* src, uint32_t* dst, uint4* scratch,
+                         const uint32_t* perm = nullptr, const uint32_t* range = nullptr) {
+  if constexpr (AffRing<T>::USED)
+    k_affine_pairs_ws<T, FIRST><<<grid, AFF_WS_THREADS, AffRing<T>::BYTES, s>>>(plan, total_ptr, src, dst, scratch, perm, range);
+  else
+    k_affine_pairs<T, FIRST><<<grid, B200_AFF_THREADS, 0, s>>>(plan, total_ptr, src, dst, scratch, perm, range);
+}
+
 }  // namespace b200

@@ -610,15 +610,12 @@ host::HXyzz<typename C::H> msm_device(Engine& E, const void* d_scalars, const vo
       static thread_local int bps_cache[MAX_DEVICES] = {};
       int bps = bps_cache[E.device];
       if (bps == 0) {
-        B200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_affine_pairs<T, true>, B200_AFF_THREADS, 0));
-        int bps2 = 0;
-        B200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps2, k_affine_pairs<T, false>, B200_AFF_THREADS, 0));
-        if (bps2 < bps) bps = bps2;
+        B200_CUDA_CHECK(affine_pairs_blocks_per_sm<T>(&bps));
         if (bps < 1) bps = 1;
         bps_cache[E.device] = bps;
       }
       const unsigned aff_grid = (unsigned)(E.sm_count * bps);
-      const size_t aff_threads = (size_t)aff_grid * B200_AFF_THREADS;
+      const size_t aff_threads = (size_t)aff_grid * affine_pairs_slot_threads<T>();
       const size_t per_thread = (level_cap(1) + aff_threads - 1) / aff_threads;
       E.aff_scratch.ensure(per_thread * aff_threads * (size_t)T::WORDS * 4);
       uint32_t* head = (uint32_t*)E.aff_head.ptr;
@@ -657,14 +654,14 @@ host::HXyzz<typename C::H> msm_device(Engine& E, const void* d_scalars, const vo
                                                           (const uint32_t*)E.part_counts.ptr, (uint32_t*)E.part_perm.ptr);
           for (int q = 0; q < PC; q++) {
             piece_ready(q);
-            k_affine_pairs<T, true><<<aff_grid, B200_AFF_THREADS, 0, s>>>(E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr,
-                                                                          (const uint32_t*)E.part_perm.ptr, (const uint32_t*)E.part_starts.ptr + q);
+            launch_affine_pairs<T, true>(aff_grid, s, E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr,
+                                         (const uint32_t*)E.part_perm.ptr, (const uint32_t*)E.part_starts.ptr + q);
           }
           launches += 3 + PC - 1;
         } else if (r == 0)
-          k_affine_pairs<T, true><<<aff_grid, B200_AFF_THREADS, 0, s>>>(E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr);
+          launch_affine_pairs<T, true>(aff_grid, s, E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr);
         else
-          k_affine_pairs<T, false><<<aff_grid, B200_AFF_THREADS, 0, s>>>(E.aff_plan[r].ptr, total_ptr, (const uint32_t*)E.aff_work[r & 1].ptr, dst, (uint4*)E.aff_scratch.ptr);
+          launch_affine_pairs<T, false>(aff_grid, s, E.aff_plan[r].ptr, total_ptr, (const uint32_t*)E.aff_work[r & 1].ptr, dst, (uint4*)E.aff_scratch.ptr);
       }
       keys = (const uint32_t*)E.keys_s.ptr;
       vals = (const uint32_t*)E.vals_s.ptr;
