@@ -158,10 +158,11 @@ void* upload_device(const void* src, size_t bytes) {
 
 void free_device(void* p) { if (p) cudaFree(p); }
 
+// prove_device's marks in E.caller_ev
+enum ProveMark { PROVE_START, PROVE_QUOTIENT_DONE };
+
 void prove_device(const void* d_points, size_t table_stride, int force_c, const void* d_roots, const uint8_t* blobs,
                   const OpeningArgs* args, size_t n, host::HXyzz<host::HFp<Bls12381Fp>>* proofs, uint64_t* y_mont, ProveTimes* times) {
-  using C = Bls12381G1;
-  using HP = host::HXyzz<typename C::H>;
   if (n == 0) return;
   EngineLease lease = acquire_engine();
   Engine& E = *lease.e;
@@ -174,19 +175,17 @@ void prove_device(const void* d_points, size_t table_stride, int force_c, const 
   uint32_t* d_y = (uint32_t*)((char*)E.kzg_args.ptr + n * sizeof(OpeningArgs));
   B200_CUDA_CHECK(cudaMemcpyAsync(E.kzg_poly.ptr, blobs, bytes, cudaMemcpyHostToDevice, s));
   B200_CUDA_CHECK(cudaMemcpyAsync(d_args, args, n * sizeof(OpeningArgs), cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[7], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[PROVE_START], s));
   k_kzg_parse<<<(unsigned)((elems + 255) / 256), 256, 0, s>>>((uint32_t*)E.kzg_poly.ptr, elems);
   k_kzg_quotient<<<(unsigned)n, KZG_THREADS, 0, s>>>((const uint32_t*)E.kzg_poly.ptr, (const uint32_t*)d_roots, d_args,
                                                      (uint32_t*)E.d_scalars.ptr, d_y);
   B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
-  E.stats.ms_h2d = 0;
-  if (n == 1) proofs[0] = msm_device<C>(E, E.d_scalars.ptr, d_points, KZG_N, /*fr_mont=*/true, force_c, 0, -1, nullptr, table_stride);
-  else {
-    std::vector<HP> res(n, HP::inf());
-    msm_device<C>(E, E.d_scalars.ptr, d_points, KZG_N, /*fr_mont=*/true, force_c, 0, -1, nullptr, table_stride, n, /*point_sets=*/1, res.data());
-    for (size_t j = 0; j < n; j++) proofs[j] = res[j];
-  }
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[PROVE_QUOTIENT_DONE], s));
+  MsmJob job(E.d_scalars.ptr, d_points, KZG_N, /*fr_mont=*/true);
+  job.force_c = force_c; job.table_stride = table_stride;
+  job.batch = n;
+  job.dest = MsmJob::HOST_ARRAY; job.out = proofs;
+  msm_device<Bls12381G1>(E, job);
   thread_stats() = E.stats;
   E.ensure_host(n * 32);
   B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, d_y, n * 32, cudaMemcpyDeviceToHost, s));
@@ -194,7 +193,7 @@ void prove_device(const void* d_points, size_t table_stride, int force_c, const 
   memcpy(y_mont, E.h_result, n * 32);
   if (times) {
     times->ms_quotient = 0;
-    cudaEventElapsedTime(&times->ms_quotient, E.ev[7], E.ev[8]);
+    cudaEventElapsedTime(&times->ms_quotient, E.caller_ev[PROVE_START], E.caller_ev[PROVE_QUOTIENT_DONE]);
   }
 }
 

@@ -174,17 +174,7 @@ int ctt_b200_bases_precompute_for(ctt_b200_bases* bases, size_t msm_len, int c) 
 }
 
 int ctt_b200_msm_cached_bases(const ctt_b200_bases* bases, int out_kind, void* r, const void* coefs, size_t len, int fr_mont) {
-  const Bases* b = reinterpret_cast<const Bases*>(bases);
-  if (!b || len > b->len) return -1;
-  const void* pts = b->d_table ? b->d_table : b->d_points;
-  const size_t stride = b->d_table ? b->len : 0;
-  const int force_c = b->d_table ? b->table_c : 0;
-  switch (b->curve_id) {
-#define X(ID, DESC) case ID: msm_cached<DESC>(r, coefs, pts, len, fr_mont != 0, out_kind, force_c, stride); return 0;
-    B200_FOR_EACH_CURVE(X)
-#undef X
-  }
-  return -1;
+  return ctt_b200_msm_batch_cached_bases(bases, out_kind, r, coefs, 1, len, fr_mont, /*shared_points=*/1);
 }
 
 int ctt_b200_msm_batch_host(int curve_id, int out_kind, void* r, const void* coefs, const void* points, size_t batch,
@@ -202,9 +192,10 @@ int ctt_b200_msm_batch_cached_bases(const ctt_b200_bases* bases, int out_kind, v
   const Bases* b = reinterpret_cast<const Bases*>(bases);
   if (!b) return -1;
   if ((shared_points ? len : batch * len) > b->len) return -1;
-  const void* pts = b->d_table ? b->d_table : b->d_points;
-  const size_t stride = b->d_table ? b->len : 0;
-  const int force_c = b->d_table ? b->table_c : 0;
+  const void* pts;
+  size_t stride;
+  int force_c;
+  bases_view(bases, &pts, &stride, &force_c);
   switch (b->curve_id) {
 #define X(ID, DESC) case ID: msm_batch_cached<DESC>(r, coefs, pts, batch, len, fr_mont != 0, out_kind, force_c, stride, shared_points != 0); return 0;
     B200_FOR_EACH_CURVE(X)

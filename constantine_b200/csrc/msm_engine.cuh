@@ -150,6 +150,11 @@ struct DeviceBuffer {
   void release() { if (ptr) cudaFree(ptr); ptr = nullptr; cap = 0; }
 };
 
+// Phase marks of msm_device: the start of the call, the start of the timed chunk's digits, then the end of each phase. Recorded by
+// msm_device and read by collect_msm_times, nothing else.
+enum MsmMark { MSM_START, MSM_CHUNK_START, MSM_DIGITS_DONE, MSM_SORT_DONE, MSM_AFFINE_DONE, MSM_ACCUMULATE_DONE, MSM_FIXUP_DONE,
+               MSM_REDUCE_DONE, MSM_DONE, MSM_MARKS };
+
 struct Engine {
   std::mutex mu;
   bool ready = false;
@@ -160,7 +165,11 @@ struct Engine {
   cudaStream_t order_after = nullptr;  // caller's stream this lease only orders itself behind (slots other than slot 0)
   cudaEvent_t ev_order = nullptr;
   cudaStream_t compute() const { return user_stream ? user_stream : stream; }
-  cudaEvent_t ev[13];
+  cudaEvent_t msm_ev[MSM_MARKS];
+  // timing events of the engine's callers (the h2d window of msm_host_on, the phases of the KZG / PeerDAS / verification drivers),
+  // each named by the caller that records it; msm_device never records them
+  static constexpr int CALLER_MARKS = 6;
+  cudaEvent_t caller_ev[CALLER_MARKS];
   cudaEvent_t ev_points_ready;
   static constexpr int MAX_INPUT_CHUNKS = 8;
   cudaEvent_t ev_chunk[MAX_INPUT_CHUNKS];
@@ -205,7 +214,8 @@ struct Engine {
     B200_CUDA_CHECK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device));
     B200_CUDA_CHECK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     B200_CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
-    for (auto& x : ev) B200_CUDA_CHECK(cudaEventCreate(&x));
+    for (auto& x : msm_ev) B200_CUDA_CHECK(cudaEventCreate(&x));
+    for (auto& x : caller_ev) B200_CUDA_CHECK(cudaEventCreate(&x));
     B200_CUDA_CHECK(cudaEventCreateWithFlags(&ev_points_ready, cudaEventDisableTiming));
     B200_CUDA_CHECK(cudaEventCreateWithFlags(&ev_order, cudaEventDisableTiming));
     for (auto& x : ev_chunk) B200_CUDA_CHECK(cudaEventCreateWithFlags(&x, cudaEventDisableTiming));
@@ -389,9 +399,9 @@ host::HXyzz<H> horner_window_digits(const host::HXyzz<H>* parts, int nw, int gro
 }
 
 // ---- one MSM on device-resident inputs ------------------------------------------------------------------------
-// d_scalars: n x 32 B, d_points: n affine points (ABI layout, Montgomery residues). Produces the window sums in pinned
-// host memory and runs the host tail. Window range [win_begin, win_end) lets several devices split one MSM by windows;
-// the returned point is then  sum_{w in range} 2^(c*w) * S_w.
+// d_scalars: n x 32 B, d_points: n affine points (ABI layout, Montgomery residues). Produces the window sums and runs the tail.
+// Window range [win_begin, win_end) lets several devices split one MSM by windows; the result is then
+// sum_{w in range} 2^(c*w) * S_w.
 // Table mode (table_stride > 0): d_points is a [W][table_stride] array holding 2^(c*w) * P_i in affine form (built by
 // precompute_table below for cached bases). Every window then drops its points into ONE shared set of 2^(c-1) buckets,
 // so the bucket reduction runs once instead of W times and the Horner tail disappears.
@@ -399,9 +409,9 @@ host::HXyzz<H> horner_window_digits(const host::HXyzz<H>* parts, int nw, int gro
 // are the bucket sets ("logical windows"), so many small MSMs (reference: banks of fixed-base PrecomputedMSM,
 // ec_multi_scalar_mul_precomp.nim:192-240 called per output in matrix/toeplitz.nim:347-360) fill the machine like one
 // large MSM does. d_scalars = batch*n scalars; d_points = point_sets*n points, MSM m using set m mod point_sets (point_sets = batch:
-// every MSM its own bases, 1: all share one set); the results are written to batch_out[0..batch) and the tail (Horner per MSM)
-// runs on the device. batch_out_device: batch_out is a DEVICE buffer that k_batch_tail writes, stream-ordered, and the call returns
-// without synchronising (the caller reads the phase times with collect_msm_times once it has synchronised the stream).
+// every MSM its own bases, 1: all share one set); the tail (Horner per MSM) runs on the device. A device destination is written by
+// k_batch_tail, stream-ordered, and the call returns without synchronising (the caller reads the phase times with
+// collect_msm_times once it has synchronised the stream).
 // Input chunks (single MSMs from host memory): the pairs arrive in consecutive chunks, each guarded by an event of the copy
 // stream. Digits, sort and bucket accumulation run per chunk INTO THE SAME buckets (a run that opens a bucket starts from
 // the bucket's current value), so the engine works on chunk k while chunk k+1 is still crossing PCIe; the bucket reduction
@@ -419,296 +429,351 @@ struct PointChunks {
   const std::function<void(int)>* stage = nullptr;
 };
 
-// Phase times of the last msm_device call on E from its events (E.ev[6] must have completed: the call synchronised, or the caller
-// synchronised the stream after a batch_out_device call).
+// One call of msm_device: its inputs, its options and where its result goes. Callers construct a job from its inputs and set the
+// options they need.
+struct MsmJob {
+  enum Dest {
+    RETURN,          // a single MSM: the point is returned (host tail)
+    HOST_ARRAY,      // `batch` points into the host array `out`; batch == 1 takes the single-MSM path and writes out[0]
+    DEVICE_ARRAY,    // batch > 1: `batch` points into the device array `out`, stream-ordered, no synchronisation
+    DEVICE_DIGITS,   // the radix-16 digits of the window sums into the device buffer `out`, no synchronisation
+  };
+  const void* d_scalars;                 // batch * n scalars of 32 B
+  const void* d_points;                  // point_sets * n affine points, or the window table
+  size_t n;                              // terms per MSM
+  bool fr_mont;                          // the scalars are Fr Montgomery residues
+  int force_c = 0;                       // window size (0: the tuning's, else the cost model's)
+  int win_begin = 0, win_end = -1;       // windows [win_begin, win_end) of a single MSM (-1: through the last)
+  cudaEvent_t wait_points = nullptr;     // the points are ready behind this event (the scalars are stream-ordered)
+  size_t table_stride = 0;               // > 0: d_points is a [W][table_stride] window table
+  size_t batch = 1, point_sets = 1;
+  const std::vector<InputChunk>* input_chunks = nullptr;   // single MSM from host memory: the pairs in chunks
+  const PointChunks* point_chunks = nullptr;               // single MSM from host memory: the points in pieces
+  Dest dest = RETURN;
+  void* out = nullptr;                   // the buffer of every destination but RETURN
+  MsmJob(const void* scalars, const void* points, size_t terms, bool mont) : d_scalars(scalars), d_points(points), n(terms), fr_mont(mont) {}
+};
+
+// Phase times of the last msm_device call on E from its marks (MSM_DONE must have completed: the call synchronised, or the caller
+// synchronised the stream after a call with a device destination).
 inline void collect_msm_times(Engine& E) {
   if (!E.collect_timing) return;
   Stats& st = E.stats;
-  cudaEventElapsedTime(&st.ms_digits, E.ev[10], E.ev[1]);
-  cudaEventElapsedTime(&st.ms_sort, E.ev[1], E.ev[2]);
-  cudaEventElapsedTime(&st.ms_accumulate, E.ev[2], E.ev[3]);
-  if (st.affine_levels) cudaEventElapsedTime(&st.ms_affine, E.ev[2], E.ev[9]);
-  cudaEventElapsedTime(&st.ms_fixup, E.ev[3], E.ev[4]);
-  cudaEventElapsedTime(&st.ms_reduce, E.ev[4], E.ev[5]);
-  cudaEventElapsedTime(&st.ms_d2h_tail, E.ev[5], E.ev[6]);
-  cudaEventElapsedTime(&st.ms_total, E.ev[0], E.ev[6]);
+  const cudaEvent_t* m = E.msm_ev;
+  cudaEventElapsedTime(&st.ms_digits, m[MSM_CHUNK_START], m[MSM_DIGITS_DONE]);
+  cudaEventElapsedTime(&st.ms_sort, m[MSM_DIGITS_DONE], m[MSM_SORT_DONE]);
+  cudaEventElapsedTime(&st.ms_accumulate, m[MSM_SORT_DONE], m[MSM_ACCUMULATE_DONE]);
+  if (st.affine_levels) cudaEventElapsedTime(&st.ms_affine, m[MSM_SORT_DONE], m[MSM_AFFINE_DONE]);
+  cudaEventElapsedTime(&st.ms_fixup, m[MSM_ACCUMULATE_DONE], m[MSM_FIXUP_DONE]);
+  cudaEventElapsedTime(&st.ms_reduce, m[MSM_FIXUP_DONE], m[MSM_REDUCE_DONE]);
+  cudaEventElapsedTime(&st.ms_d2h_tail, m[MSM_REDUCE_DONE], m[MSM_DONE]);
+  cudaEventElapsedTime(&st.ms_total, m[MSM_START], m[MSM_DONE]);
 }
 
-template <class C>
-host::HXyzz<typename C::H> msm_device(Engine& E, const void* d_scalars, const void* d_points, size_t n, bool fr_mont,
-                                      int force_c, int win_begin, int win_end, cudaEvent_t wait_points = nullptr,
-                                      size_t table_stride = 0, size_t batch = 1, size_t point_sets = 1,
-                                      host::HXyzz<typename C::H>* batch_out = nullptr,
-                                      const std::vector<InputChunk>* input_chunks = nullptr, void* d_digits_out = nullptr,
-                                      const PointChunks* point_chunks = nullptr, bool batch_out_device = false) {
-  using T = typename C::T;
-  using H = typename C::H;
-  using HP = host::HXyzz<H>;
-  constexpr int KFIX = 32;   // fix-up slice length
-  Stats& st = E.stats;
-  int launches = 0;
-  if (batch == 0) return HP::inf();
-  if (n == 0) {
-    if (batch_out) for (size_t m = 0; m < batch; m++) batch_out[m] = HP::inf();
-    return HP::inf();
-  }
-  if (batch * n >= (1ull << 31)) { fprintf(stderr, "[ctt_b200_msm] FATAL: len >= 2^31 unsupported\n"); abort(); }
-  if (batch > 1 && (batch_out == nullptr || win_begin != 0 || win_end >= 0 || point_sets < 1 || point_sets > batch)) {
-    fprintf(stderr, "[ctt_b200_msm] FATAL: a batch takes all windows and needs an output array\n"); abort();
-  }
-  const bool table_mode = table_stride > 0;
-  if (input_chunks && (batch > 1 || table_mode || input_chunks->empty())) input_chunks = nullptr;
+// The jobs msm_device refuses (the interface has no error channel: a refusal aborts with its reason).
+[[noreturn]] inline void refuse(const char* why) { fprintf(stderr, "[ctt_b200_msm] FATAL: %s\n", why); abort(); }
+inline void check_job(const Engine& E, const MsmJob& job) {
+  if (job.batch * job.n >= (1ull << 31)) refuse("len >= 2^31 unsupported");
+  if (job.batch > 1 && (job.dest == MsmJob::RETURN || job.win_begin != 0 || job.win_end >= 0 || job.point_sets < 1 || job.point_sets > job.batch))
+    refuse("a batch takes all windows and needs an output array");
+  if (job.dest != MsmJob::RETURN && !job.out) refuse("the destination of the result has no buffer");
+  if (job.dest == MsmJob::DEVICE_ARRAY && job.batch == 1) refuse("a device array of results needs a batch (batch > 1)");
+  if (job.dest == MsmJob::DEVICE_DIGITS && (job.batch != 1 || E.tuning.reduce_mode != 0))
+    refuse("device digits need the bit-plane reduction (single MSM, reduce mode 0)");
+  if (job.input_chunks && job.point_chunks) refuse("input chunks and point pieces exclude each other");
+}
 
-  int c = force_c > 0 ? force_c : (E.tuning.force_c > 0 ? E.tuning.force_c : choose_window(n, C::SCALAR_BITS, T::WORDS));
+// Sizes of one call, derived from its job and the engine's tuning.
+struct MsmSizes {
+  int c = 0;
+  DigitPlan plan;
+  int nwd = 0;                 // digit windows handled by this call
+  int nws = 0;                 // bucket sets per MSM (table mode: 1)
+  int nw = 0;                  // bucket sets of the call ("logical windows"): batch * nws
+  uint32_t B = 0;              // buckets per set
+  size_t nbuckets = 0;
+  uint32_t no_key = 0;         // key of the zero digits: sorts after every bucket
+  bool table_mode = false;
+  bool plane_reduce = false;   // bit-plane bucket reduction (single MSMs), else running-sum chunks
+};
+
+template <class C>
+MsmSizes msm_sizes(const Engine& E, const MsmJob& job) {
+  MsmSizes z;
+  z.table_mode = job.table_stride > 0;
+  z.plane_reduce = job.batch == 1 && E.tuning.reduce_mode == 0;
+  int c = job.force_c > 0 ? job.force_c : (E.tuning.force_c > 0 ? E.tuning.force_c : choose_window(job.n, C::SCALAR_BITS, C::T::WORDS));
   if (c < 2) c = 2;
   if (c > 20) c = 20;
-  DigitPlan plan = make_plan(C::SCALAR_BITS, c, win_begin, win_end);
-  const int nwd = plan.win_end - plan.win_begin;          // digit windows handled by this call
-  if (nwd <= 0) return HP::inf();
-  const int nws = table_mode ? 1 : nwd;                   // bucket sets per MSM
-  const size_t nw_total = batch * (size_t)nws;            // bucket sets ("logical windows") of the call
-  if (table_mode && (size_t)nwd * table_stride >= (1ull << 31)) { fprintf(stderr, "[ctt_b200_msm] FATAL: table too large\n"); abort(); }
-  const uint32_t B = plan.buckets_per_window;
-  const size_t nbuckets = nw_total * B;
-  if (nbuckets >= 0xFFFFFFF0ull || nw_total >= (1ull << 30) || (size_t)nwd * batch * n >= (1ull << 32)) {
-    fprintf(stderr, "[ctt_b200_msm] FATAL: batch too large for 32-bit bucket keys\n"); abort();
-  }
-  const int nw = (int)nw_total;
-  const uint32_t no_key = (uint32_t)nbuckets;
-  constexpr size_t XYZZ_BYTES = 4 * T::WORDS * 4;
-  constexpr size_t XW = 4 * T::WORDS;  // 32-bit words per XYZZ point
+  z.c = c;
+  z.plan = make_plan(C::SCALAR_BITS, c, job.win_begin, job.win_end);
+  z.nwd = z.plan.win_end - z.plan.win_begin;
+  if (z.nwd <= 0) return z;
+  z.nws = z.table_mode ? 1 : z.nwd;
+  const size_t nw_total = job.batch * (size_t)z.nws;
+  if (z.table_mode && (size_t)z.nwd * job.table_stride >= (1ull << 31)) refuse("table too large");
+  z.B = z.plan.buckets_per_window;
+  z.nbuckets = nw_total * z.B;
+  if (z.nbuckets >= 0xFFFFFFF0ull || nw_total >= (1ull << 30) || (size_t)z.nwd * job.batch * job.n >= (1ull << 32))
+    refuse("batch too large for 32-bit bucket keys");
+  z.nw = (int)nw_total;
+  z.no_key = (uint32_t)z.nbuckets;
+  return z;
+}
+
+// The compute stream waits for the points of a host call: every piece of `pc` (PC > 0; the host-side staging of a piece, if any,
+// runs here), else the event `ready` if there is one.
+inline void wait_piece(cudaStream_t s, const PointChunks& pc, int q) {
+  if (pc.stage && *pc.stage) (*pc.stage)(q);
+  B200_CUDA_CHECK(cudaStreamWaitEvent(s, pc.ready[q], 0));
+}
+inline void wait_points(cudaStream_t s, int PC, const PointChunks* pc, cudaEvent_t ready) {
+  if (PC) { for (int q = 0; q < PC; q++) wait_piece(s, *pc, q); }
+  else if (ready) B200_CUDA_CHECK(cudaStreamWaitEvent(s, ready, 0));
+}
+
+// Batched-affine levels of one chunk: run bounds, level offsets and pair lists from the sorted keys, then AL levels of pair
+// additions. keys / vals / acc_points become the survivor list that k_accumulate walks.
+template <class C>
+void affine_levels(Engine& E, const MsmSizes& z, int AL, size_t entries, size_t acc_entries, size_t nper, const void* pts, int PC,
+                   const PointChunks* pc, cudaEvent_t points_ready, bool timed, const uint32_t*& keys, const uint32_t*& vals,
+                   const void*& acc_points, int& launches) {
+  using T = typename C::T;
   constexpr size_t AFF_BYTES = 2 * T::WORDS * 4;
-  st.c = c; st.num_windows = nwd; st.total_buckets = nbuckets; st.ms_affine = 0; st.entries = 0; st.groups = 1;
+  cudaStream_t s = E.compute();
+  auto level_cap = [&](int r) { return (entries >> r) + z.nbuckets + 1; };   // level r holds sum_b ceil(n_b / 2^r) <= this many slots
+  const uint32_t nb = (uint32_t)z.nbuckets;
+  const uint32_t nblk = (nb + SCAN_ITEMS - 1) / SCAN_ITEMS;
+  const size_t off_stride = (size_t)nb + 1;
+  E.aff_head.ensure((size_t)nb * 4); E.aff_tail.ensure((size_t)nb * 4);
+  E.aff_off.ensure((size_t)(AL + 1) * off_stride * 4);
+  E.aff_blocksum.ensure((size_t)(AL + 1) * nblk * 4);
+  E.aff_plan[0].ensure(level_cap(1) * 8);
+  for (int r = 1; r < AL; r++) E.aff_plan[r].ensure(level_cap(r + 1) * 4);
+  E.aff_work[1].ensure(level_cap(1) * AFF_BYTES);               // odd levels
+  if (AL >= 2) E.aff_work[0].ensure(level_cap(2) * AFF_BYTES);  // even levels
+  E.keys_s.ensure(acc_entries * 4);
+  E.vals_s.ensure(acc_entries * 4);
+  // persistent grid of the pair kernel: as many blocks as stay resident (queried once per curve and device: the query
+  // costs tens of microseconds of host time per call, which would stall the launch queue of every MSM)
+  static thread_local int bps_cache[MAX_DEVICES] = {};
+  int bps = bps_cache[E.device];
+  if (bps == 0) {
+    B200_CUDA_CHECK(affine_pairs_blocks_per_sm<T>(&bps));
+    if (bps < 1) bps = 1;
+    bps_cache[E.device] = bps;
+  }
+  const unsigned aff_grid = (unsigned)(E.sm_count * bps);
+  const size_t aff_threads = (size_t)aff_grid * affine_pairs_slot_threads<T>();
+  const size_t per_thread = (level_cap(1) + aff_threads - 1) / aff_threads;
+  E.aff_scratch.ensure(per_thread * aff_threads * (size_t)T::WORDS * 4);
+  uint32_t* head = (uint32_t*)E.aff_head.ptr;
+  uint32_t* tail = (uint32_t*)E.aff_tail.ptr;
+  uint32_t* off = (uint32_t*)E.aff_off.ptr;
+  B200_CUDA_CHECK(cudaMemsetAsync(head, 0, (size_t)nb * 4, s));
+  B200_CUDA_CHECK(cudaMemsetAsync(tail, 0, (size_t)nb * 4, s));
+  B200_CUDA_CHECK(cudaMemsetAsync(E.keys_s.ptr, 0xFF, acc_entries * 4, s));   // KEY_NONE: the unused tail sorts last, like zero digits
+  const unsigned eb = (unsigned)((entries + 255) / 256);
+  k_bucket_bounds<<<eb, 256, 0, s>>>(keys, entries, z.no_key, head, tail);
+  k_level_blocksums<<<nblk, SCAN_THREADS, 0, s>>>(head, tail, nb, AL, nblk, (uint32_t*)E.aff_blocksum.ptr);
+  k_level_scan<<<1, SCAN_THREADS, 0, s>>>((uint32_t*)E.aff_blocksum.ptr, nblk, AL, nb, off);
+  k_level_offsets<<<nblk, SCAN_THREADS, 0, s>>>(head, tail, nb, AL, nblk, (const uint32_t*)E.aff_blocksum.ptr, off);
+  AffinePlan aplan;
+  aplan.plan0 = (uint2*)E.aff_plan[0].ptr;
+  for (int r = 0; r < AFF_MAX_LEVELS; r++) aplan.plan[r] = (r >= 1 && r < AL) ? (uint32_t*)E.aff_plan[r].ptr : nullptr;
+  aplan.surv_keys = (uint32_t*)E.keys_s.ptr;
+  aplan.surv_vals = (uint32_t*)E.vals_s.ptr;
+  k_affine_plan<<<eb, 256, 0, s>>>(keys, vals, entries, z.no_key, head, tail, off, nb, AL, aplan);
+  const bool split0 = PC > 1;
+  if (!split0) wait_points(s, PC, pc, points_ready);
+  for (int r = 0; r < AL; r++) {
+    const uint32_t* total_ptr = off + (size_t)(r + 1) * off_stride + nb;      // size of level r + 1
+    uint32_t* dst = (uint32_t*)E.aff_work[(r + 1) & 1].ptr;
+    if (r == 0 && split0) {
+      // level 0 by arrival of the point pieces: stable partition of the pair list by the last piece a pair touches, one launch
+      // per piece behind that piece's event (k_part_* in msm_affine.cuh)
+      const uint32_t Pq = (uint32_t)PC;
+      const uint32_t nblk_p = (uint32_t)((level_cap(1) + PART_TILE - 1) / PART_TILE);
+      E.part_counts.ensure((size_t)Pq * nblk_p * 4);
+      E.part_starts.ensure((size_t)(Pq + 1) * 4);
+      E.part_perm.ensure(level_cap(1) * 4);
+      k_part_count<<<nblk_p, PART_THREADS, 0, s>>>((const uint2*)E.aff_plan[0].ptr, total_ptr, (uint32_t)nper, Pq, nblk_p, (uint32_t*)E.part_counts.ptr);
+      k_part_scan<<<1, SCAN_THREADS, 0, s>>>((uint32_t*)E.part_counts.ptr, Pq, nblk_p, (uint32_t*)E.part_starts.ptr);
+      k_part_scatter<<<nblk_p, PART_THREADS, 0, s>>>((const uint2*)E.aff_plan[0].ptr, total_ptr, (uint32_t)nper, Pq, nblk_p,
+                                                      (const uint32_t*)E.part_counts.ptr, (uint32_t*)E.part_perm.ptr);
+      for (int q = 0; q < PC; q++) {
+        wait_piece(s, *pc, q);
+        launch_affine_pairs<T, true>(aff_grid, s, E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr,
+                                     (const uint32_t*)E.part_perm.ptr, (const uint32_t*)E.part_starts.ptr + q);
+      }
+      launches += 3 + PC - 1;
+    } else if (r == 0)
+      launch_affine_pairs<T, true>(aff_grid, s, E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr);
+    else
+      launch_affine_pairs<T, false>(aff_grid, s, E.aff_plan[r].ptr, total_ptr, (const uint32_t*)E.aff_work[r & 1].ptr, dst, (uint4*)E.aff_scratch.ptr);
+  }
+  keys = (const uint32_t*)E.keys_s.ptr;
+  vals = (const uint32_t*)E.vals_s.ptr;
+  acc_points = E.aff_work[AL & 1].ptr;
+  k_window_bounds<<<(unsigned)((z.nw + 1 + 63) / 64), 64, 0, s>>>(keys, acc_entries, z.B, z.nw, (unsigned long long*)E.bounds.ptr);
+  launches += 6 + AL;
+  B200_CUDA_CHECK(cudaGetLastError());
+  if (timed) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_AFFINE_DONE], s));
+}
+
+// Front half of one input chunk, into the buckets: digits -> sort -> (batched-affine levels) -> XYZZ slices -> fix-up. `chunked`: the
+// job's input chunks are in use; `into`: the buckets already hold the sums of the earlier chunks; `timed`: this chunk records the
+// phase marks (the last, or only, chunk).
+template <class C>
+void msm_chunk(Engine& E, const MsmJob& job, const MsmSizes& z, const InputChunk& ch, bool chunked, bool into, bool timed, int& launches) {
+  using T = typename C::T;
+  constexpr int KFIX = 32;   // fix-up slice length
+  constexpr size_t XYZZ_BYTES = 4 * T::WORDS * 4;
+  constexpr size_t AFF_BYTES = 2 * T::WORDS * 4;
+  Stats& st = E.stats;
+  cudaStream_t s = E.compute();
+  const size_t nper = ch.count;                           // terms per MSM in this chunk (batches are never chunked)
+  const size_t ntot = job.batch * nper;
+  const size_t entries = (size_t)z.nwd * ntot;
+  const void* sc = (const char*)job.d_scalars + ch.begin * 32;
+  const void* pts = z.table_mode ? job.d_points : (const void*)((const char*)job.d_points + ch.begin * AFF_BYTES);
+  st.entries += entries;
+
+  // batched-affine levels: the XYZZ accumulation then runs over the survivor list only
+  int AL = E.tuning.affine_levels;
+  if (AL < 0) AL = auto_affine_levels(entries, z.nbuckets, job.batch, T::WORDS);
+  if (entries >= (1ull << 31) || z.nbuckets >= (1ull << 30)) AL = 0;
+  if (AL > AFF_MAX_LEVELS) AL = AFF_MAX_LEVELS;
+  const size_t acc_entries = AL ? (entries >> AL) + z.nbuckets + 1 : entries;   // upper bound of the list k_accumulate walks (level AL)
+  // slice length of k_accumulate. Every thread of a resident wave walks one slice, so the kernel's time is (waves) x (slice
+  // length) whatever the fill of the last wave: the slices are sized to fill a whole number of waves, on the device, from the
+  // actual entry count (accumulate_slice_len in msm_kernels.cuh; fixed lengths 16 / 32 / 64 differ by their wave counts). KACC is the upper limit: longer slices mean fewer
+  // partial sums for k_fixup but coarser balance. tuning.slice_len > 0 fixes the length instead (sweeps), < 0 sets the limit.
+  int KACC = 64;
+  uint32_t fit_threads;
+  {
+    static thread_local int acc_bps_cache[MAX_DEVICES] = {};
+    int bps = acc_bps_cache[E.device];
+    if (bps == 0) {
+      B200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_accumulate<T>, B200_ACC_THREADS, 0));
+      if (bps < 1) bps = 1;
+      acc_bps_cache[E.device] = bps;
+    }
+    fit_threads = (uint32_t)(E.sm_count * bps * B200_ACC_THREADS);
+    if (E.tuning.slice_len > 0) { KACC = E.tuning.slice_len; fit_threads = 0; }
+    else if (E.tuning.slice_len < 0) KACC = -E.tuning.slice_len;
+  }
+  st.slice_len = fit_threads ? accumulate_slice_len(acc_entries, fit_threads, KACC) : KACC;   // (fitted: for the upper bound of the list)
+  E.keys_a.ensure(entries * 4); E.keys_b.ensure(entries * 4);
+  E.vals_a.ensure(entries * 4); E.vals_b.ensure(entries * 4);
+  if (timed) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_CHUNK_START], s));
+  // 1. digits (need the chunk's scalars only when they come over the compute stream; chunked input: wait for the chunk)
+  if (chunked && ch.ready) B200_CUDA_CHECK(cudaStreamWaitEvent(s, ch.ready, 0));
+  {
+    dim3 grid((unsigned)((ntot + 255) / 256)), block(256);
+    const uint32_t msm_key_stride = (uint32_t)z.nws * z.B, psets = job.batch > 1 ? (uint32_t)job.point_sets : 1u;
+    if (job.fr_mont)
+      k_digits<typename C::FrParams, true><<<grid, block, 0, s>>>((const uint32_t*)sc, (uint32_t)ntot, z.plan, (uint32_t*)E.keys_a.ptr, (uint32_t*)E.vals_a.ptr,
+                                                                   z.table_mode ? 0u : z.B, z.no_key, (uint32_t)job.table_stride, (uint32_t)nper, msm_key_stride, psets);
+    else
+      k_digits<typename C::FrParams, false><<<grid, block, 0, s>>>((const uint32_t*)sc, (uint32_t)ntot, z.plan, (uint32_t*)E.keys_a.ptr, (uint32_t*)E.vals_a.ptr,
+                                                                    z.table_mode ? 0u : z.B, z.no_key, (uint32_t)job.table_stride, (uint32_t)nper, msm_key_stride, psets);
+    launches++;
+  }
+  if (timed) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_DIGITS_DONE], s));
+  // 2. sort by key
+  int end_bit = 1;
+  while ((1ull << end_bit) <= (unsigned long long)z.no_key) end_bit++;
+  cub::DoubleBuffer<uint32_t> dk((uint32_t*)E.keys_a.ptr, (uint32_t*)E.keys_b.ptr);
+  cub::DoubleBuffer<uint32_t> dv((uint32_t*)E.vals_a.ptr, (uint32_t*)E.vals_b.ptr);
+  {
+    size_t tmp_bytes = 0;
+    B200_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, dk, dv, (int64_t)entries, 0, end_bit, s));
+    E.cub_tmp.ensure(tmp_bytes);
+    B200_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(E.cub_tmp.ptr, tmp_bytes, dk, dv, (int64_t)entries, 0, end_bit, s));
+    launches += 2 + (end_bit + 7) / 8;  // histogram + exclusive-sum + one onesweep pass per 8 key bits
+  }
+  const uint32_t* keys = dk.Current();
+  const uint32_t* vals = dv.Current();
+  if (timed) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_SORT_DONE], s));
+  E.bounds.ensure((size_t)(z.nw + 1) * 8);
+  k_window_bounds<<<(unsigned)((z.nw + 1 + 63) / 64), 64, 0, s>>>(keys, entries, z.B, z.nw, (unsigned long long*)E.bounds.ptr);
+  launches++;
+  // slices (upper bounds known on the host; the exact entry ranges stay on the device)
+  size_t max_slices;
+  {
+    size_t set_cap = z.table_mode ? (size_t)z.nwd * nper : nper;   // a bucket set holds <= n (table: nwd * n) entries
+    if (AL) set_cap = (set_cap >> AL) + z.B + 1;                   // ... of which ceil(run / 2^AL) per bucket survive the affine levels
+    const size_t list_cap = (size_t)z.nw * set_cap;
+    max_slices = fit_threads ? accumulate_waves(list_cap, fit_threads, KACC) * fit_threads : (list_cap + KACC - 1) / KACC;
+  }
+  const size_t max_fix = (max_slices + KFIX - 1) / KFIX;
+  E.part_pts[0].ensure(max_slices * XYZZ_BYTES); E.part_keys[0].ensure(max_slices * 4);
+  E.part_pts[1].ensure(max_fix * XYZZ_BYTES); E.part_keys[1].ensure(max_fix * 4);
+  // points of a host call arrive on the copy stream: nothing up to here reads them, and neither does the batched-affine plan
+  // (run bounds, level offsets, pair lists come from the sorted keys / refs alone), so the wait sits right in front of
+  // the first kernel that gathers points.
+  // Point pieces of a host call (`point_chunks`): the host-side staging of a piece, if any, runs HERE in the call sequence, i.e. after
+  // digits, sort and plan have been queued, and the engine waits for piece q only in front of the work that needs it.
+  const int PC = job.point_chunks ? job.point_chunks->P : 0;
+  const cudaEvent_t points_ready = chunked ? nullptr : ch.ready;   // a chunk's event was waited for before its digits
+  const void* acc_points = pts;
+  if (AL) affine_levels<C>(E, z, AL, entries, acc_entries, nper, pts, PC, job.point_chunks, points_ready, timed, keys, vals, acc_points, launches);
+  st.affine_levels = AL;
+  if (!AL) wait_points(s, PC, job.point_chunks, points_ready);
+  // 3. accumulate
+  {
+    dim3 block(B200_ACC_THREADS), grid((unsigned)((max_slices + B200_ACC_THREADS - 1) / B200_ACC_THREADS));
+    k_accumulate<T><<<grid, block, 0, s>>>(keys, vals, (const unsigned long long*)E.bounds.ptr, 0, z.nw, z.no_key, (const uint32_t*)acc_points,
+                                           (uint32_t*)E.buckets.ptr, (uint32_t*)E.part_pts[0].ptr, (uint32_t*)E.part_keys[0].ptr, max_slices, KACC,
+                                           into ? 1 : 0, fit_threads);
+    launches++;
+  }
+  if (timed) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_ACCUMULATE_DONE], s));
+  // 4. fix-up levels
+  {
+    size_t count = max_slices;
+    int cur = 0;
+    while (count > 1) {
+      size_t ns = (count + KFIX - 1) / KFIX;
+      dim3 block(128), grid((unsigned)((count + 127) / 128));
+      k_fixup<T><<<grid, block, 0, s>>>((const uint32_t*)E.part_keys[cur].ptr, (const uint32_t*)E.part_pts[cur].ptr, count,
+                                        (uint32_t*)E.buckets.ptr, (uint32_t*)E.part_pts[cur ^ 1].ptr, (uint32_t*)E.part_keys[cur ^ 1].ptr);
+      launches++;
+      count = ns;
+      cur ^= 1;
+    }
+    // the last level is a single chunk: its first entry has no predecessor, so nothing is forwarded any further
+  }
+  if (timed) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_FIXUP_DONE], s));
+}
+
+// Where the bucket reduction left its results: `per_set` points per bucket set at `parts`. Bit-plane: the radix-16 digits of each
+// window sum (in red_planes); running-sum: the partial sums of each set (<= 4 for a single MSM, 1 for a batch) in red_a or red_b.
+struct Reduced {
+  const void* parts;
+  uint32_t per_set;
+};
+
 #ifndef B200_INLINE_MAX_WORDS
 #define B200_INLINE_MAX_WORDS 12
 #endif
+
+template <class C>
+Reduced reduce_buckets(Engine& E, const MsmSizes& z, size_t batch, int& launches) {
+  using T = typename C::T;
+  constexpr size_t XYZZ_BYTES = 4 * T::WORDS * 4;
+  constexpr size_t XW = 4 * T::WORDS;  // 32-bit words per XYZZ point
   constexpr bool INL = (T::WORDS <= B200_INLINE_MAX_WORDS);   // single-field coordinates: inline the point adds; Fp2: out-of-line (code size)
   cudaStream_t s = E.compute();
-  E.buckets.ensure(nbuckets * XYZZ_BYTES);
-  if (E.collect_timing) B200_CUDA_CHECK(cudaEventRecord(E.ev[0], s));
-  B200_CUDA_CHECK(cudaMemsetAsync(E.buckets.ptr, 0, nbuckets * XYZZ_BYTES, s));  // all-zero XYZZ = infinity
-
-  // ================= front half, once per input chunk: digits -> sort -> (batched-affine levels) -> XYZZ slices -> fix-up
-  const std::vector<InputChunk> whole = {InputChunk{0, n, wait_points}};
-  const std::vector<InputChunk>& chunks_in = input_chunks ? *input_chunks : whole;
-  for (size_t ck = 0; ck < chunks_in.size(); ck++) {
-    const InputChunk& ch = chunks_in[ck];
-    if (ch.count == 0) continue;
-    const bool into = ck > 0;                               // buckets already hold the sums of the earlier chunks
-    const bool last_chunk = ck + 1 == chunks_in.size();
-    const bool timed = E.collect_timing && last_chunk;      // phase times: those of the last (or only) chunk
-    const size_t nper = ch.count;                           // terms per MSM in this chunk (batches are never chunked)
-    const size_t ntot = batch * nper;
-    const size_t entries = (size_t)nwd * ntot;
-    const void* sc = (const char*)d_scalars + ch.begin * 32;
-    const void* pts = table_mode ? d_points : (const void*)((const char*)d_points + ch.begin * AFF_BYTES);
-    st.entries += entries;
-
-    // batched-affine levels: the XYZZ accumulation then runs over the survivor list only
-    int AL = E.tuning.affine_levels;
-    if (AL < 0) AL = auto_affine_levels(entries, nbuckets, batch, T::WORDS);
-    if (entries >= (1ull << 31) || nbuckets >= (1ull << 30)) AL = 0;
-    if (AL > AFF_MAX_LEVELS) AL = AFF_MAX_LEVELS;
-    // level r holds sum_b ceil(n_b / 2^r) <= entries / 2^r + nbuckets slots
-    auto level_cap = [&](int r) { return (entries >> r) + nbuckets + 1; };
-    const size_t acc_entries = AL ? level_cap(AL) : entries;   // upper bound of the list k_accumulate walks
-    // slice length of k_accumulate. Every thread of a resident wave walks one slice, so the kernel's time is (waves) x (slice
-    // length) whatever the fill of the last wave: the slices are sized to fill a whole number of waves, on the device, from the
-    // actual entry count (accumulate_slice_len in msm_kernels.cuh; fixed lengths 16 / 32 / 64 differ by their wave counts). KACC is the upper limit: longer slices mean fewer
-    // partial sums for k_fixup but coarser balance. tuning.slice_len > 0 fixes the length instead (sweeps), < 0 sets the limit.
-    int KACC = 64;
-    uint32_t fit_threads;
-    {
-      static thread_local int acc_bps_cache[MAX_DEVICES] = {};
-      int bps = acc_bps_cache[E.device];
-      if (bps == 0) {
-        B200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_accumulate<T>, B200_ACC_THREADS, 0));
-        if (bps < 1) bps = 1;
-        acc_bps_cache[E.device] = bps;
-      }
-      fit_threads = (uint32_t)(E.sm_count * bps * B200_ACC_THREADS);
-      if (E.tuning.slice_len > 0) { KACC = E.tuning.slice_len; fit_threads = 0; }
-      else if (E.tuning.slice_len < 0) KACC = -E.tuning.slice_len;
-    }
-    st.slice_len = fit_threads ? accumulate_slice_len(acc_entries, fit_threads, KACC) : KACC;   // (fitted: for the upper bound of the list)
-    E.keys_a.ensure(entries * 4); E.keys_b.ensure(entries * 4);
-    E.vals_a.ensure(entries * 4); E.vals_b.ensure(entries * 4);
-    if (timed) B200_CUDA_CHECK(cudaEventRecord(E.ev[10], s));
-    // 1. digits (need the chunk's scalars only when they come over the compute stream; chunked input: wait for the chunk)
-    if (input_chunks && ch.ready) B200_CUDA_CHECK(cudaStreamWaitEvent(s, ch.ready, 0));
-    {
-      dim3 grid((unsigned)((ntot + 255) / 256)), block(256);
-      const uint32_t msm_key_stride = (uint32_t)nws * B, psets = batch > 1 ? (uint32_t)point_sets : 1u;
-      if (fr_mont)
-        k_digits<typename C::FrParams, true><<<grid, block, 0, s>>>((const uint32_t*)sc, (uint32_t)ntot, plan, (uint32_t*)E.keys_a.ptr, (uint32_t*)E.vals_a.ptr,
-                                                                     table_mode ? 0u : B, no_key, (uint32_t)table_stride, (uint32_t)nper, msm_key_stride, psets);
-      else
-        k_digits<typename C::FrParams, false><<<grid, block, 0, s>>>((const uint32_t*)sc, (uint32_t)ntot, plan, (uint32_t*)E.keys_a.ptr, (uint32_t*)E.vals_a.ptr,
-                                                                      table_mode ? 0u : B, no_key, (uint32_t)table_stride, (uint32_t)nper, msm_key_stride, psets);
-      launches++;
-    }
-    if (timed) B200_CUDA_CHECK(cudaEventRecord(E.ev[1], s));
-    // 2. sort by key
-    int end_bit = 1;
-    while ((1ull << end_bit) <= (unsigned long long)no_key) end_bit++;
-    cub::DoubleBuffer<uint32_t> dk((uint32_t*)E.keys_a.ptr, (uint32_t*)E.keys_b.ptr);
-    cub::DoubleBuffer<uint32_t> dv((uint32_t*)E.vals_a.ptr, (uint32_t*)E.vals_b.ptr);
-    {
-      size_t tmp_bytes = 0;
-      B200_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, dk, dv, (int64_t)entries, 0, end_bit, s));
-      E.cub_tmp.ensure(tmp_bytes);
-      B200_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(E.cub_tmp.ptr, tmp_bytes, dk, dv, (int64_t)entries, 0, end_bit, s));
-      launches += 2 + (end_bit + 7) / 8;  // histogram + exclusive-sum + one onesweep pass per 8 key bits
-    }
-    const uint32_t* keys = dk.Current();
-    const uint32_t* vals = dv.Current();
-    if (timed) B200_CUDA_CHECK(cudaEventRecord(E.ev[2], s));
-    E.bounds.ensure((size_t)(nw + 1) * 8);
-    k_window_bounds<<<(unsigned)((nw + 1 + 63) / 64), 64, 0, s>>>(keys, entries, B, nw, (unsigned long long*)E.bounds.ptr);
-    launches++;
-    // slices (upper bounds known on the host; the exact entry ranges stay on the device)
-    size_t max_slices;
-    {
-      size_t set_cap = table_mode ? (size_t)nwd * nper : nper;   // a bucket set holds <= n (table: nwd * n) entries
-      if (AL) set_cap = (set_cap >> AL) + B + 1;                 // ... of which ceil(run / 2^AL) per bucket survive the affine levels
-      const size_t list_cap = (size_t)nw * set_cap;
-      max_slices = fit_threads ? accumulate_waves(list_cap, fit_threads, KACC) * fit_threads : (list_cap + KACC - 1) / KACC;
-    }
-    const size_t max_fix = (max_slices + KFIX - 1) / KFIX;
-    E.part_pts[0].ensure(max_slices * XYZZ_BYTES); E.part_keys[0].ensure(max_slices * 4);
-    E.part_pts[1].ensure(max_fix * XYZZ_BYTES); E.part_keys[1].ensure(max_fix * 4);
-    // points of a host call arrive on the copy stream: nothing up to here reads them, and neither does the batched-affine plan
-    // below (run bounds, level offsets, pair lists come from the sorted keys / refs alone), so the wait sits right in front of
-    // the first kernel that gathers points
-    // Point pieces of a host call (`point_chunks`): the host-side staging of a piece, if any, runs HERE in the call sequence, i.e. after
-    // digits, sort and plan have been queued, and the engine waits for piece q only in front of the work that needs it.
-    const int PC = (point_chunks && !input_chunks) ? point_chunks->P : 0;
-    auto piece_ready = [&](int q) {
-      if (point_chunks->stage && *point_chunks->stage) (*point_chunks->stage)(q);
-      B200_CUDA_CHECK(cudaStreamWaitEvent(s, point_chunks->ready[q], 0));
-    };
-    auto wait_for_points = [&]() {
-      if (PC) { for (int q = 0; q < PC; q++) piece_ready(q); }
-      else if (!input_chunks && ch.ready) B200_CUDA_CHECK(cudaStreamWaitEvent(s, ch.ready, 0));
-    };
-    const void* acc_points = pts;
-    if (AL) {
-      const uint32_t nb = (uint32_t)nbuckets;
-      const uint32_t nblk = (nb + SCAN_ITEMS - 1) / SCAN_ITEMS;
-      const size_t off_stride = (size_t)nb + 1;
-      E.aff_head.ensure((size_t)nb * 4); E.aff_tail.ensure((size_t)nb * 4);
-      E.aff_off.ensure((size_t)(AL + 1) * off_stride * 4);
-      E.aff_blocksum.ensure((size_t)(AL + 1) * nblk * 4);
-      E.aff_plan[0].ensure(level_cap(1) * 8);
-      for (int r = 1; r < AL; r++) E.aff_plan[r].ensure(level_cap(r + 1) * 4);
-      E.aff_work[1].ensure(level_cap(1) * AFF_BYTES);               // odd levels
-      if (AL >= 2) E.aff_work[0].ensure(level_cap(2) * AFF_BYTES);  // even levels
-      E.keys_s.ensure(acc_entries * 4);
-      E.vals_s.ensure(acc_entries * 4);
-      // persistent grid of the pair kernel: as many blocks as stay resident (queried once per curve and device: the query
-      // costs tens of microseconds of host time per call, which would stall the launch queue of every MSM)
-      static thread_local int bps_cache[MAX_DEVICES] = {};
-      int bps = bps_cache[E.device];
-      if (bps == 0) {
-        B200_CUDA_CHECK(affine_pairs_blocks_per_sm<T>(&bps));
-        if (bps < 1) bps = 1;
-        bps_cache[E.device] = bps;
-      }
-      const unsigned aff_grid = (unsigned)(E.sm_count * bps);
-      const size_t aff_threads = (size_t)aff_grid * affine_pairs_slot_threads<T>();
-      const size_t per_thread = (level_cap(1) + aff_threads - 1) / aff_threads;
-      E.aff_scratch.ensure(per_thread * aff_threads * (size_t)T::WORDS * 4);
-      uint32_t* head = (uint32_t*)E.aff_head.ptr;
-      uint32_t* tail = (uint32_t*)E.aff_tail.ptr;
-      uint32_t* off = (uint32_t*)E.aff_off.ptr;
-      B200_CUDA_CHECK(cudaMemsetAsync(head, 0, (size_t)nb * 4, s));
-      B200_CUDA_CHECK(cudaMemsetAsync(tail, 0, (size_t)nb * 4, s));
-      B200_CUDA_CHECK(cudaMemsetAsync(E.keys_s.ptr, 0xFF, acc_entries * 4, s));   // KEY_NONE: the unused tail sorts last, like zero digits
-      const unsigned eb = (unsigned)((entries + 255) / 256);
-      k_bucket_bounds<<<eb, 256, 0, s>>>(keys, entries, no_key, head, tail);
-      k_level_blocksums<<<nblk, SCAN_THREADS, 0, s>>>(head, tail, nb, AL, nblk, (uint32_t*)E.aff_blocksum.ptr);
-      k_level_scan<<<1, SCAN_THREADS, 0, s>>>((uint32_t*)E.aff_blocksum.ptr, nblk, AL, nb, off);
-      k_level_offsets<<<nblk, SCAN_THREADS, 0, s>>>(head, tail, nb, AL, nblk, (const uint32_t*)E.aff_blocksum.ptr, off);
-      AffinePlan aplan;
-      aplan.plan0 = (uint2*)E.aff_plan[0].ptr;
-      for (int r = 0; r < AFF_MAX_LEVELS; r++) aplan.plan[r] = (r >= 1 && r < AL) ? (uint32_t*)E.aff_plan[r].ptr : nullptr;
-      aplan.surv_keys = (uint32_t*)E.keys_s.ptr;
-      aplan.surv_vals = (uint32_t*)E.vals_s.ptr;
-      k_affine_plan<<<eb, 256, 0, s>>>(keys, vals, entries, no_key, head, tail, off, nb, AL, aplan);
-      const bool split0 = PC > 1;
-      if (!split0) wait_for_points();
-      for (int r = 0; r < AL; r++) {
-        const uint32_t* total_ptr = off + (size_t)(r + 1) * off_stride + nb;      // size of level r + 1
-        uint32_t* dst = (uint32_t*)E.aff_work[(r + 1) & 1].ptr;
-        if (r == 0 && split0) {
-          // level 0 by arrival of the point pieces: stable partition of the pair list by the last piece a pair touches, one launch
-          // per piece behind that piece's event (k_part_* in msm_affine.cuh)
-          const uint32_t Pq = (uint32_t)PC;
-          const uint32_t nblk_p = (uint32_t)((level_cap(1) + PART_TILE - 1) / PART_TILE);
-          E.part_counts.ensure((size_t)Pq * nblk_p * 4);
-          E.part_starts.ensure((size_t)(Pq + 1) * 4);
-          E.part_perm.ensure(level_cap(1) * 4);
-          k_part_count<<<nblk_p, PART_THREADS, 0, s>>>((const uint2*)E.aff_plan[0].ptr, total_ptr, (uint32_t)nper, Pq, nblk_p, (uint32_t*)E.part_counts.ptr);
-          k_part_scan<<<1, SCAN_THREADS, 0, s>>>((uint32_t*)E.part_counts.ptr, Pq, nblk_p, (uint32_t*)E.part_starts.ptr);
-          k_part_scatter<<<nblk_p, PART_THREADS, 0, s>>>((const uint2*)E.aff_plan[0].ptr, total_ptr, (uint32_t)nper, Pq, nblk_p,
-                                                          (const uint32_t*)E.part_counts.ptr, (uint32_t*)E.part_perm.ptr);
-          for (int q = 0; q < PC; q++) {
-            piece_ready(q);
-            launch_affine_pairs<T, true>(aff_grid, s, E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr,
-                                         (const uint32_t*)E.part_perm.ptr, (const uint32_t*)E.part_starts.ptr + q);
-          }
-          launches += 3 + PC - 1;
-        } else if (r == 0)
-          launch_affine_pairs<T, true>(aff_grid, s, E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr);
-        else
-          launch_affine_pairs<T, false>(aff_grid, s, E.aff_plan[r].ptr, total_ptr, (const uint32_t*)E.aff_work[r & 1].ptr, dst, (uint4*)E.aff_scratch.ptr);
-      }
-      keys = (const uint32_t*)E.keys_s.ptr;
-      vals = (const uint32_t*)E.vals_s.ptr;
-      acc_points = E.aff_work[AL & 1].ptr;
-      k_window_bounds<<<(unsigned)((nw + 1 + 63) / 64), 64, 0, s>>>(keys, acc_entries, B, nw, (unsigned long long*)E.bounds.ptr);
-      launches += 6 + AL;
-      B200_CUDA_CHECK(cudaGetLastError());
-      if (timed) B200_CUDA_CHECK(cudaEventRecord(E.ev[9], s));
-    }
-    st.affine_levels = AL;
-    if (!AL) wait_for_points();
-    // 3. accumulate
-    {
-      dim3 block(B200_ACC_THREADS), grid((unsigned)((max_slices + B200_ACC_THREADS - 1) / B200_ACC_THREADS));
-      k_accumulate<T><<<grid, block, 0, s>>>(keys, vals, (const unsigned long long*)E.bounds.ptr, 0, nw, no_key, (const uint32_t*)acc_points,
-                                             (uint32_t*)E.buckets.ptr, (uint32_t*)E.part_pts[0].ptr, (uint32_t*)E.part_keys[0].ptr, max_slices, KACC,
-                                             into ? 1 : 0, fit_threads);
-      launches++;
-    }
-    if (timed) B200_CUDA_CHECK(cudaEventRecord(E.ev[3], s));
-    // 4. fix-up levels
-    {
-      size_t count = max_slices;
-      int cur = 0;
-      while (count > 1) {
-        size_t ns = (count + KFIX - 1) / KFIX;
-        dim3 block(128), grid((unsigned)((count + 127) / 128));
-        k_fixup<T><<<grid, block, 0, s>>>((const uint32_t*)E.part_keys[cur].ptr, (const uint32_t*)E.part_pts[cur].ptr, count,
-                                          (uint32_t*)E.buckets.ptr, (uint32_t*)E.part_pts[cur ^ 1].ptr, (uint32_t*)E.part_keys[cur ^ 1].ptr);
-        launches++;
-        count = ns;
-        cur ^= 1;
-      }
-      // the last level is a single chunk: its first entry has no predecessor, so nothing is forwarded any further
-    }
-    if (timed) B200_CUDA_CHECK(cudaEventRecord(E.ev[4], s));
-  }
-
-  // ================= back half, once: bucket reduction and tail
-  // bit-plane reduction (single MSMs): buckets as a 2^rbits x 2^a matrix per window, see k_rowcol_sums
-  const bool plane_reduce = (batch == 1 && E.tuning.reduce_mode == 0);
-  const int pr_a = (c - 1) / 2, pr_rbits = (c - 1) - pr_a;
-  const uint32_t pr_planes = (uint32_t)(c - 1);                 // bit positions 0 .. c-2 of the bucket weights j + 1 = h*C + (l+1) (k_plane_sums)
-  const uint32_t pr_groups = (pr_planes + 3) / 4;               // radix-16 digits per window handed to the host
-  uint32_t row = 0;
-  DeviceBuffer* src = &E.red_a;
-  if (plane_reduce) {
+  const int c = z.c, nw = z.nw;
+  const uint32_t B = z.B;
+  const size_t nbuckets = z.nbuckets;
+  if (z.plane_reduce) {
+    // bit-plane reduction (single MSMs): buckets as a 2^rbits x 2^a matrix per window, see k_rowcol_sums
+    const int pr_a = (c - 1) / 2, pr_rbits = (c - 1) - pr_a;
+    const uint32_t pr_planes = (uint32_t)(c - 1);                 // bit positions 0 .. c-2 of the bucket weights j + 1 = h*C + (l+1) (k_plane_sums)
+    const uint32_t pr_groups = (pr_planes + 3) / 4;               // radix-16 digits per window handed to the host
     const uint32_t Cn = 1u << pr_a, Rn = 1u << pr_rbits;
     // terms summed serially by one lane: as many as keep >= ~8 warps per SM busy, at least 2
 #ifndef B200_REDUCE_THREADS_PER_SM
@@ -740,109 +805,143 @@ host::HXyzz<typename C::H> msm_device(Engine& E, const void* d_scalars, const vo
                                                                       (uint32_t)nw, lanes_p, planes_ptr);
     k_plane_combine<T, INL><<<(unsigned)(((size_t)nw * pr_groups * 4 + 63) / 64), 64, 0, s>>>(planes_ptr, pr_planes, pr_groups, (uint32_t)nw, digits_ptr);
     launches += 3;
-  } else {
-    // running-sum chunks, offsets, warp-butterfly row sums (<= 4 per window left; batches: one)
-    uint32_t L = (uint32_t)E.tuning.reduce_chunk;
-    if (L < 1) L = 1;
-    uint32_t chunks = (B + L - 1) / L;
-    // small bucket counts: the phase is a chain of dependent point operations, so trade chunk length for more threads
-    // (a larger target for Fp2 was measured slower: the offset multiplication per chunk dominates then)
-    const size_t want_threads = (size_t)E.sm_count * 64;
-    while (L > 1 && (size_t)chunks * nw < want_threads && chunks < B) { L = (L + 1) / 2; chunks = (B + L - 1) / L; }
-    int nbits = 0;
-    while (nbits < 32 && ((uint64_t)(chunks - 1) * L >> nbits) != 0) nbits++;
-    E.red_a.ensure((size_t)chunks * nw * XYZZ_BYTES);
-    E.red_b.ensure((size_t)chunks * nw * XYZZ_BYTES);
-    size_t threads = (size_t)chunks * nw;
-    dim3 block(64), grid((unsigned)((threads + 63) / 64));
-    k_bucket_reduce<T, INL><<<grid, block, 0, s>>>((const uint32_t*)E.buckets.ptr, B, L, chunks, (uint32_t)nw, (uint32_t*)E.red_a.ptr, (uint32_t*)E.red_b.ptr);
-    k_chunk_offset<T, INL><<<grid, block, 0, s>>>((uint32_t*)E.red_a.ptr, (const uint32_t*)E.red_b.ptr, L, chunks, (uint32_t)nw, nbits);
-    launches += 2;
-    row = chunks;
-    bool in_a = true;
-    // single MSM: <= 4 partial sums per window go to the host tail; batch: down to one, the device tail is a serial chain
-    const uint32_t row_stop = batch > 1 ? 1u : 4u;
-    while (row > row_stop) {
-      uint32_t out_row = (row + 31) / 32;
-      size_t warps = (size_t)out_row * nw;
-      dim3 blk(128), grd((unsigned)((warps * 32 + 127) / 128));
-      k_row_sum_warp<T, INL><<<grd, blk, 0, s>>>((const uint32_t*)(in_a ? E.red_a.ptr : E.red_b.ptr), row, out_row, (uint32_t)nw,
-                                                 (uint32_t*)(in_a ? E.red_b.ptr : E.red_a.ptr));
-      launches++;
-      row = out_row;
-      in_a = !in_a;
-    }
-    src = in_a ? &E.red_a : &E.red_b;
+    return Reduced{digits_ptr, pr_groups};
   }
-  if (E.collect_timing) B200_CUDA_CHECK(cudaEventRecord(E.ev[5], s));
-  static_assert(sizeof(HP) == XYZZ_BYTES, "host/device XYZZ layout");
-  if (d_digits_out) {
-    // multi-GPU window sharding: leave this device's radix-16 window digits in the caller's DEVICE buffer and return without
-    // synchronising -- the caller's collective (same stream) gathers every rank's digits and ONE host pass combines them
-    if (!plane_reduce) { fprintf(stderr, "[ctt_b200_msm] FATAL: device digits need the bit-plane reduction (single MSM, reduce mode 0)\n"); abort(); }
-    B200_CUDA_CHECK(cudaMemcpyAsync(d_digits_out, (const uint32_t*)E.red_planes.ptr + (size_t)nw * pr_planes * XW, (size_t)nw * pr_groups * XYZZ_BYTES,
-                                    cudaMemcpyDeviceToDevice, s));
-    st.kernel_launches = launches;
-    st.ms_total = 0;
-    return HP::inf();
+  // running-sum chunks, offsets, warp-butterfly row sums (<= 4 per window left; batches: one)
+  uint32_t L = (uint32_t)E.tuning.reduce_chunk;
+  if (L < 1) L = 1;
+  uint32_t chunks = (B + L - 1) / L;
+  // small bucket counts: the phase is a chain of dependent point operations, so trade chunk length for more threads
+  // (a larger target for Fp2 was measured slower: the offset multiplication per chunk dominates then)
+  const size_t want_threads = (size_t)E.sm_count * 64;
+  while (L > 1 && (size_t)chunks * nw < want_threads && chunks < B) { L = (L + 1) / 2; chunks = (B + L - 1) / L; }
+  int nbits = 0;
+  while (nbits < 32 && ((uint64_t)(chunks - 1) * L >> nbits) != 0) nbits++;
+  E.red_a.ensure((size_t)chunks * nw * XYZZ_BYTES);
+  E.red_b.ensure((size_t)chunks * nw * XYZZ_BYTES);
+  size_t threads = (size_t)chunks * nw;
+  dim3 block(64), grid((unsigned)((threads + 63) / 64));
+  k_bucket_reduce<T, INL><<<grid, block, 0, s>>>((const uint32_t*)E.buckets.ptr, B, L, chunks, (uint32_t)nw, (uint32_t*)E.red_a.ptr, (uint32_t*)E.red_b.ptr);
+  k_chunk_offset<T, INL><<<grid, block, 0, s>>>((uint32_t*)E.red_a.ptr, (const uint32_t*)E.red_b.ptr, L, chunks, (uint32_t)nw, nbits);
+  launches += 2;
+  uint32_t row = chunks;
+  bool in_a = true;
+  // single MSM: <= 4 partial sums per window go to the host tail; batch: down to one, the device tail is a serial chain
+  const uint32_t row_stop = batch > 1 ? 1u : 4u;
+  while (row > row_stop) {
+    uint32_t out_row = (row + 31) / 32;
+    size_t warps = (size_t)out_row * nw;
+    dim3 blk(128), grd((unsigned)((warps * 32 + 127) / 128));
+    k_row_sum_warp<T, INL><<<grd, blk, 0, s>>>((const uint32_t*)(in_a ? E.red_a.ptr : E.red_b.ptr), row, out_row, (uint32_t)nw,
+                                               (uint32_t*)(in_a ? E.red_b.ptr : E.red_a.ptr));
+    launches++;
+    row = out_row;
+    in_a = !in_a;
   }
-  auto read_times = [&]() {
-    if (!E.collect_timing) return;
-    B200_CUDA_CHECK(cudaEventRecord(E.ev[6], s));
-    B200_CUDA_CHECK(cudaEventSynchronize(E.ev[6]));
-    collect_msm_times(E);
+  return Reduced{in_a ? E.red_a.ptr : E.red_b.ptr, row};
+}
+
+// Single MSM: the per-window results to the host and the tail there. r = sum_w 2^(c*w) S_w  for w in [win_begin, win_end): Horner
+// over the bit positions (reference ec_multi_scalar_mul_parallel.nim:198-203: c doublings + one addition per window), including
+// the shift by c*win_begin.
+template <class C>
+host::HXyzz<typename C::H> host_tail(Engine& E, const MsmSizes& z, const Reduced& red) {
+  using HP = host::HXyzz<typename C::H>;
+  static_assert(sizeof(HP) == 4 * C::T::WORDS * 4, "host/device XYZZ layout");
+  cudaStream_t s = E.compute();
+  const size_t out_bytes = (size_t)z.nw * red.per_set * sizeof(HP);
+  E.ensure_host(out_bytes);
+  B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, red.parts, out_bytes, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  const HP* parts = reinterpret_cast<const HP*>(E.h_result);
+  // bit-plane: window w arrives as radix-16 digits D_g of its sum, S_w = sum_g 16^g D_g
+  if (z.plane_reduce) return horner_window_digits<typename C::H>(parts, z.nw, (int)red.per_set, z.c, z.table_mode ? 0 : z.plan.win_begin);
+  // running-sum: <= 4 partial sums per window, finished here
+  const uint32_t row = red.per_set;
+  auto window_sum = [&](int w) {
+    HP a = parts[(size_t)w * row];
+    for (uint32_t i = 1; i < row; i++) a = host::xyzz_add(a, parts[(size_t)w * row + i]);
+    return a;
   };
-  if (batch > 1 && batch_out_device) {
-    // 6c. batch left on the device: the tail writes the caller's buffer; no copy, no synchronisation
-    k_batch_tail<T><<<(unsigned)((batch + 63) / 64), 64, 0, s>>>((const uint32_t*)src->ptr, row, nws, c, (uint32_t)batch, (uint32_t*)batch_out);
-    launches++;
-    if (E.collect_timing) B200_CUDA_CHECK(cudaEventRecord(E.ev[6], s));
-    st.kernel_launches = launches;
+  HP r = window_sum(z.nw - 1);
+  for (int w = z.nw - 2; w >= 0; w--) {
+    for (int i = 0; i < z.c; i++) r = host::xyzz_dbl(r);
+    r = host::xyzz_add(r, window_sum(w));
+  }
+  for (int i = 0; i < z.c * z.plan.win_begin; i++) r = host::xyzz_dbl(r);
+  return r;
+}
+
+// The end mark once the call's work is queued; waits for it and reads the phase times
+inline void finish_times(Engine& E) {
+  if (!E.collect_timing) return;
+  B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_DONE], E.compute()));
+  B200_CUDA_CHECK(cudaEventSynchronize(E.msm_ev[MSM_DONE]));
+  collect_msm_times(E);
+}
+
+// Runs `job` on E's compute stream: the front half once per input chunk, the bucket reduction, then the exit of the job's destination.
+// Returns the point of a single MSM (the neutral element for the other destinations).
+template <class C>
+host::HXyzz<typename C::H> msm_device(Engine& E, const MsmJob& job) {
+  using HP = host::HXyzz<typename C::H>;
+  constexpr size_t XYZZ_BYTES = sizeof(HP);
+  check_job(E, job);
+  Stats& st = E.stats;
+  st.ms_h2d = 0;   // a host call sets its own after this
+  if (job.batch == 0) return HP::inf();
+  if (job.n == 0) {
+    if (job.dest == MsmJob::HOST_ARRAY) for (size_t m = 0; m < job.batch; m++) static_cast<HP*>(job.out)[m] = HP::inf();
     return HP::inf();
   }
-  if (batch > 1) {
-    // 6b. batch: partial sums + Horner per MSM on the device (one thread per MSM), then `batch` points -> host
-    DeviceBuffer* dst = (src == &E.red_a) ? &E.red_b : &E.red_a;   // the other reduce buffer is free by now (>= nw points)
-    k_batch_tail<T><<<(unsigned)((batch + 63) / 64), 64, 0, s>>>((const uint32_t*)src->ptr, row, nws, c, (uint32_t)batch, (uint32_t*)dst->ptr);
-    launches++;
-    E.ensure_host(batch * XYZZ_BYTES);
-    B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, dst->ptr, batch * XYZZ_BYTES, cudaMemcpyDeviceToHost, s));
-    B200_CUDA_CHECK(cudaStreamSynchronize(s));
-    memcpy((void*)batch_out, E.h_result, batch * XYZZ_BYTES);
-    read_times();
-    st.kernel_launches = launches;
-    return HP::inf();
+  const MsmSizes z = msm_sizes<C>(E, job);
+  if (z.nwd <= 0) return HP::inf();
+  st.c = z.c; st.num_windows = z.nwd; st.total_buckets = z.nbuckets; st.ms_affine = 0; st.entries = 0; st.groups = 1;
+  int launches = 0;
+  cudaStream_t s = E.compute();
+  E.buckets.ensure(z.nbuckets * XYZZ_BYTES);
+  if (E.collect_timing) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_START], s));
+  B200_CUDA_CHECK(cudaMemsetAsync(E.buckets.ptr, 0, z.nbuckets * XYZZ_BYTES, s));  // all-zero XYZZ = infinity
+
+  const bool chunked = job.input_chunks && !job.input_chunks->empty() && job.batch == 1 && !z.table_mode;
+  const std::vector<InputChunk> whole = {InputChunk{0, job.n, job.wait_points}};
+  const std::vector<InputChunk>& chunks = chunked ? *job.input_chunks : whole;
+  for (size_t ck = 0; ck < chunks.size(); ck++) {
+    if (chunks[ck].count == 0) continue;
+    const bool timed = E.collect_timing && ck + 1 == chunks.size();   // phase times: those of the last (or only) chunk
+    msm_chunk<C>(E, job, z, chunks[ck], chunked, ck > 0, timed, launches);
   }
-  // 6. host tail. r = sum_w 2^(c*w) S_w  for w in [win_begin, win_end): Horner over the bit positions (reference
-  // ec_multi_scalar_mul_parallel.nim:198-203: c doublings + one addition per window), including the shift by c*win_begin.
+  const Reduced red = reduce_buckets<C>(E, z, job.batch, launches);
+  if (E.collect_timing) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_REDUCE_DONE], s));
+
   HP r = HP::inf();
-  if (plane_reduce) {
-    // window w arrives as radix-16 digits D_g of its sum, S_w = sum_g 16^g D_g
-    const size_t out_bytes = (size_t)nw * pr_groups * XYZZ_BYTES;
-    E.ensure_host(out_bytes);
-    B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, (const uint32_t*)E.red_planes.ptr + (size_t)nw * pr_planes * XW, out_bytes, cudaMemcpyDeviceToHost, s));
-    B200_CUDA_CHECK(cudaStreamSynchronize(s));
-    r = horner_window_digits<H>(reinterpret_cast<const HP*>(E.h_result), nw, (int)pr_groups, c, table_mode ? 0 : plan.win_begin);
-  } else {
-    // per-window partial sums (<= 4 each) -> host; finish the sums there
-    const size_t out_bytes = (size_t)nw * row * XYZZ_BYTES;
-    E.ensure_host(out_bytes);
-    B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, src->ptr, out_bytes, cudaMemcpyDeviceToHost, s));
-    B200_CUDA_CHECK(cudaStreamSynchronize(s));
-    const HP* parts = reinterpret_cast<const HP*>(E.h_result);
-    auto window_sum = [&](int w) {
-      HP a = parts[(size_t)w * row];
-      for (uint32_t i = 1; i < row; i++) a = host::xyzz_add(a, parts[(size_t)w * row + i]);
-      return a;
-    };
-    r = window_sum(nw - 1);
-    for (int w = nw - 2; w >= 0; w--) {
-      for (int i = 0; i < c; i++) r = host::xyzz_dbl(r);
-      r = host::xyzz_add(r, window_sum(w));
+  if (job.dest == MsmJob::DEVICE_DIGITS) {
+    // multi-GPU window sharding: this device's radix-16 window digits stay in the caller's DEVICE buffer, no synchronisation --
+    // the caller's collective (same stream) gathers every rank's digits and ONE host pass combines them
+    B200_CUDA_CHECK(cudaMemcpyAsync(job.out, red.parts, (size_t)z.nw * red.per_set * XYZZ_BYTES, cudaMemcpyDeviceToDevice, s));
+    st.ms_total = 0;
+  } else if (job.batch > 1) {
+    // batch: the partial sums + Horner per MSM on the device (one thread per MSM), into the caller's device array or, for the host,
+    // into the other reduce buffer (free by now, >= nw points)
+    const bool on_device = job.dest == MsmJob::DEVICE_ARRAY;
+    void* dst = on_device ? job.out : (red.parts == E.red_a.ptr ? E.red_b.ptr : E.red_a.ptr);
+    k_batch_tail<typename C::T><<<(unsigned)((job.batch + 63) / 64), 64, 0, s>>>((const uint32_t*)red.parts, red.per_set, z.nws, z.c,
+                                                                              (uint32_t)job.batch, (uint32_t*)dst);
+    launches++;
+    if (on_device) {
+      if (E.collect_timing) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_DONE], s));
+    } else {
+      E.ensure_host(job.batch * XYZZ_BYTES);
+      B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, dst, job.batch * XYZZ_BYTES, cudaMemcpyDeviceToHost, s));
+      B200_CUDA_CHECK(cudaStreamSynchronize(s));
+      memcpy(job.out, E.h_result, job.batch * XYZZ_BYTES);
+      finish_times(E);
     }
-    for (int i = 0; i < c * plan.win_begin; i++) r = host::xyzz_dbl(r);
+  } else {
+    r = host_tail<C>(E, z, red);
+    finish_times(E);
+    if (job.dest == MsmJob::HOST_ARRAY) static_cast<HP*>(job.out)[0] = r;
   }
-  read_times();
   st.kernel_launches = launches;
   return r;
 }
@@ -971,7 +1070,8 @@ host::HXyzz<typename C::H> msm_host_on(int device, const void* coefs, const void
   const size_t sbytes = len * 32, pbytes = len * (size_t)(2 * C::COORD_BYTES);
   E.d_scalars.ensure(sbytes);
   E.d_points.ensure(pbytes);
-  cudaEvent_t t0 = E.ev[7], t1 = E.ev[8];
+  enum { H2D_START, H2D_DONE };   // this call's marks in E.caller_ev
+  cudaEvent_t t0 = E.caller_ev[H2D_START], t1 = E.caller_ev[H2D_DONE];
   B200_CUDA_CHECK(cudaEventRecord(t0, E.compute()));
   // One piece (default): scalars on the compute stream (digits + sort need only them), points on the copy stream beside them.
   // Chunked (ctt_b200_set_input_chunks): scalars and points of chunk k, then chunk k+1, all on the copy stream; the engine
@@ -981,6 +1081,7 @@ host::HXyzz<typename C::H> msm_host_on(int device, const void* coefs, const void
   int P = E.tuning.input_chunks;
   if (P <= 0) P = 1;
   if (P > Engine::MAX_INPUT_CHUNKS) P = Engine::MAX_INPUT_CHUNKS;
+  MsmJob job(E.d_scalars.ptr, E.d_points.ptr, len, fr_mont);
   HP r;
   if (P > 1) {
     std::vector<InputChunk> chunks((size_t)P);
@@ -992,8 +1093,9 @@ host::HXyzz<typename C::H> msm_host_on(int device, const void* coefs, const void
       B200_CUDA_CHECK(cudaMemcpyAsync((char*)E.d_points.ptr + lo * pt, (const char*)points + lo * pt, (hi - lo) * pt, cudaMemcpyHostToDevice, E.copy_stream));
       B200_CUDA_CHECK(cudaEventRecord(E.ev_chunk[k], E.copy_stream));
     }
+    job.input_chunks = &chunks;
     B200_CUDA_CHECK(cudaEventRecord(t1, E.compute()));
-    r = msm_device<C>(E, E.d_scalars.ptr, E.d_points.ptr, len, fr_mont, 0, 0, -1, nullptr, 0, 1, 1, nullptr, &chunks);
+    r = msm_device<C>(E, job);
   } else {
     // One piece of scalars, the points in PQ pieces by point index. Pinned caller memory: scalars on the compute stream (digits + sort
     // need only them), every piece of points queued on the copy stream now with an event behind it. Pageable caller memory (what a C /
@@ -1038,8 +1140,9 @@ host::HXyzz<typename C::H> msm_host_on(int device, const void* coefs, const void
         B200_CUDA_CHECK(cudaEventRecord(E.ev_chunk[q], E.copy_stream));
       }
     }
+    job.point_chunks = &pc;
     B200_CUDA_CHECK(cudaEventRecord(t1, E.compute()));
-    r = msm_device<C>(E, E.d_scalars.ptr, E.d_points.ptr, len, fr_mont, 0, 0, -1, nullptr, 0, 1, 1, nullptr, nullptr, nullptr, &pc);
+    r = msm_device<C>(E, job);
   }
   if (E.collect_timing) cudaEventElapsedTime(&E.stats.ms_h2d, t0, t1);
   if (stats_out) *stats_out = E.stats;
@@ -1187,9 +1290,11 @@ void msm_dev_ptrs(void* r_out, const void* d_coefs, const void* d_points, size_t
                   int win_begin, int win_end, size_t table_stride) {
   EngineLease lease = acquire_engine();
   Engine& E = *lease.e;
-  using HP = host::HXyzz<typename C::H>;
-  E.stats.ms_h2d = 0;
-  HP r = msm_device<C>(E, d_coefs, d_points, len, fr_mont, force_c, win_begin, win_end, nullptr, table_stride);
+  MsmJob job(d_coefs, d_points, len, fr_mont);
+  job.force_c = force_c;
+  job.win_begin = win_begin; job.win_end = win_end;
+  job.table_stride = table_stride;
+  const auto r = msm_device<C>(E, job);
   thread_stats() = E.stats;
   write_result<C>(r_out, r, kind);
 }
@@ -1201,8 +1306,11 @@ int msm_dev_digits(void* d_digits_out, const void* d_coefs, const void* d_points
                    int win_end) {
   EngineLease lease = acquire_engine();
   Engine& E = *lease.e;
-  E.stats.ms_h2d = 0;
-  msm_device<C>(E, d_coefs, d_points, len, fr_mont, force_c, win_begin, win_end, nullptr, 0, 1, 1, nullptr, nullptr, d_digits_out);
+  MsmJob job(d_coefs, d_points, len, fr_mont);
+  job.force_c = force_c;
+  job.win_begin = win_begin; job.win_end = win_end;
+  job.dest = MsmJob::DEVICE_DIGITS; job.out = d_digits_out;
+  msm_device<C>(E, job);
   thread_stats() = E.stats;
   return (E.stats.c - 1 + 3) / 4;
 }
@@ -1213,21 +1321,6 @@ void combine_window_digits(void* r_out, const void* h_digits, int c, int num_win
   using HP = host::HXyzz<typename C::H>;
   const int groups = (c - 1 + 3) / 4;
   HP r = horner_window_digits<typename C::H>(reinterpret_cast<const HP*>(h_digits), num_windows, groups, c, 0);
-  write_result<C>(r_out, r, kind);
-}
-
-// cached bases: scalars come from the host, points (or their window table) are resident; one lease covers copy + MSM
-template <class C>
-void msm_cached(void* r_out, const void* coefs, const void* d_points, size_t len, bool fr_mont, int kind, int force_c,
-                size_t table_stride) {
-  EngineLease lease = acquire_engine();
-  Engine& E = *lease.e;
-  using HP = host::HXyzz<typename C::H>;
-  E.d_scalars.ensure(len * 32 + 16);
-  B200_CUDA_CHECK(cudaMemcpyAsync(E.d_scalars.ptr, coefs, len * 32, cudaMemcpyHostToDevice, E.compute()));
-  E.stats.ms_h2d = 0;
-  HP r = msm_device<C>(E, E.d_scalars.ptr, d_points, len, fr_mont, force_c, 0, -1, nullptr, table_stride);
-  thread_stats() = E.stats;
   write_result<C>(r_out, r, kind);
 }
 
@@ -1255,14 +1348,17 @@ void msm_batch_host(void* r_out, const void* coefs, const void* points, size_t b
   B200_CUDA_CHECK(cudaMemcpyAsync(E.d_scalars.ptr, coefs, sbytes, cudaMemcpyHostToDevice, E.compute()));
   B200_CUDA_CHECK(cudaMemcpyAsync(E.d_points.ptr, points, pbytes, cudaMemcpyHostToDevice, E.copy_stream));
   B200_CUDA_CHECK(cudaEventRecord(E.ev_points_ready, E.copy_stream));
-  E.stats.ms_h2d = 0;
-  if (batch == 1) res[0] = msm_device<C>(E, E.d_scalars.ptr, E.d_points.ptr, len, fr_mont, 0, 0, -1, E.ev_points_ready);
-  else msm_device<C>(E, E.d_scalars.ptr, E.d_points.ptr, len, fr_mont, 0, 0, -1, E.ev_points_ready, 0, batch, shared_points ? 1 : batch, res.data());
+  MsmJob job(E.d_scalars.ptr, E.d_points.ptr, len, fr_mont);
+  job.wait_points = E.ev_points_ready;
+  job.batch = batch; job.point_sets = shared_points ? 1 : batch;
+  job.dest = MsmJob::HOST_ARRAY; job.out = res.data();
+  msm_device<C>(E, job);
   thread_stats() = E.stats;
   write_results<C>(r_out, res, kind);
 }
 
-// cached bases: d_points (or the window table with row length table_stride) resident, scalars from the host
+// cached bases: d_points (or the window table with row length table_stride) resident, scalars from the host; one lease covers
+// copy + MSM
 template <class C>
 void msm_batch_cached(void* r_out, const void* coefs, const void* d_points, size_t batch, size_t len, bool fr_mont, int kind,
                       int force_c, size_t table_stride, bool shared_points) {
@@ -1274,9 +1370,11 @@ void msm_batch_cached(void* r_out, const void* coefs, const void* d_points, size
   Engine& E = *lease.e;
   E.d_scalars.ensure(batch * len * 32 + 16);
   B200_CUDA_CHECK(cudaMemcpyAsync(E.d_scalars.ptr, coefs, batch * len * 32, cudaMemcpyHostToDevice, E.compute()));
-  E.stats.ms_h2d = 0;
-  if (batch == 1) res[0] = msm_device<C>(E, E.d_scalars.ptr, d_points, len, fr_mont, force_c, 0, -1, nullptr, table_stride);
-  else msm_device<C>(E, E.d_scalars.ptr, d_points, len, fr_mont, force_c, 0, -1, nullptr, table_stride, batch, shared_points ? 1 : batch, res.data());
+  MsmJob job(E.d_scalars.ptr, d_points, len, fr_mont);
+  job.force_c = force_c; job.table_stride = table_stride;
+  job.batch = batch; job.point_sets = shared_points ? 1 : batch;
+  job.dest = MsmJob::HOST_ARRAY; job.out = res.data();
+  msm_device<C>(E, job);
   thread_stats() = E.stats;
   write_results<C>(r_out, res, kind);
 }

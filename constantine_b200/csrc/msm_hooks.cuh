@@ -204,7 +204,6 @@ void* run_precompute_table(const void* d_points, size_t n, int c, int* W_out) {
   template int msm_dev_digits<DESC>(void*, const void*, const void*, size_t, bool, int, int, int);               \
   template void combine_window_digits<DESC>(void*, const void*, int, int, int);                                  \
   template void* run_precompute_table<DESC>(const void*, size_t, int, int*);                                      \
-  template void msm_cached<DESC>(void*, const void*, const void*, size_t, bool, int, int, size_t);                \
   template void msm_batch_host<DESC>(void*, const void*, const void*, size_t, size_t, bool, int, bool);           \
   template void msm_batch_cached<DESC>(void*, const void*, const void*, size_t, size_t, bool, int, int, size_t, bool); \
   template void sum_reduce_host<DESC>(void*, const void*, size_t, int);                                           \
@@ -217,7 +216,6 @@ void* run_precompute_table(const void* d_points, size_t n, int c, int* W_out) {
   extern template int msm_dev_digits<DESC>(void*, const void*, const void*, size_t, bool, int, int, int);        \
   extern template void combine_window_digits<DESC>(void*, const void*, int, int, int);                           \
   extern template void* run_precompute_table<DESC>(const void*, size_t, int, int*);                               \
-  extern template void msm_cached<DESC>(void*, const void*, const void*, size_t, bool, int, int, size_t);         \
   extern template void msm_batch_host<DESC>(void*, const void*, const void*, size_t, size_t, bool, int, bool);    \
   extern template void msm_batch_cached<DESC>(void*, const void*, const void*, size_t, size_t, bool, int, int, size_t, bool); \
   extern template void sum_reduce_host<DESC>(void*, const void*, size_t, int);                                    \

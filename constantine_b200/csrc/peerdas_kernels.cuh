@@ -418,28 +418,32 @@ static void das_smem_opt_in(int device) {
 
 constexpr size_t DAS_XYZZ_BYTES = 4 * G1T::WORDS * 4;
 
-// The FK20 proofs of n blobs whose coefficients 0..4095 are in E.das_coefs, queued on E's stream: k_das_circulants (then ev[8]), the
-// bank MSM (then ev[11]), k_ec_fft128 (then ev[12]). The n x 128 raw XYZZ proofs are left in E.das_proofs.
+// The PeerDAS drivers' marks in E.caller_ev, each at the end of its phase but DAS_START
+enum DasMark { DAS_START, DAS_FR_DONE, DAS_MSM_DONE, DAS_ECFFT_DONE };
+
+// The FK20 proofs of n blobs whose coefficients 0..4095 are in E.das_coefs, queued on E's stream: k_das_circulants (then DAS_FR_DONE),
+// the bank MSM (then DAS_MSM_DONE), k_ec_fft128 (then DAS_ECFFT_DONE). The n x 128 raw XYZZ proofs are left in E.das_proofs.
 static void das_fk20(Engine& E, const uint32_t* tw, const DasBank& bank, size_t n) {
-  using C = Bls12381G1;
   cudaStream_t s = E.compute();
   const size_t nmsm = n * DAS_CDS;
   E.d_scalars.ensure(nmsm * DAS_L * 32 + 16);
   k_das_circulants<<<(unsigned)(2 * n), DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((const uint32_t*)E.das_coefs.ptr, tw, (uint32_t*)E.d_scalars.ptr);
   B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[DAS_FR_DONE], s));
   E.das_u.ensure(nmsm * DAS_XYZZ_BYTES);
   E.das_proofs.ensure(nmsm * DAS_XYZZ_BYTES);
-  E.stats.ms_h2d = 0;
-  msm_device<C>(E, E.d_scalars.ptr, bank.d_points, DAS_L, /*fr_mont=*/true, bank.force_c, 0, -1, nullptr, bank.table_stride, nmsm,
-                /*point_sets=*/DAS_CDS, (host::HXyzz<typename C::H>*)E.das_u.ptr, nullptr, nullptr, nullptr, /*batch_out_device=*/true);
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[11], s));
+  MsmJob job(E.d_scalars.ptr, bank.d_points, DAS_L, /*fr_mont=*/true);
+  job.force_c = bank.force_c; job.table_stride = bank.table_stride;
+  job.batch = nmsm; job.point_sets = DAS_CDS;
+  job.dest = MsmJob::DEVICE_ARRAY; job.out = E.das_u.ptr;
+  msm_device<Bls12381G1>(E, job);
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[DAS_MSM_DONE], s));
   k_ec_fft128<true><<<(unsigned)n, DAS_EC_THREADS, 0, s>>>((const uint32_t*)E.das_u.ptr, tw, (uint32_t*)E.das_proofs.ptr);
   B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[12], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[DAS_ECFFT_DONE], s));
 }
 
-// After the stream has synchronised: the MSM's phase times, and the call's device phases (ev[7] marks the start of the Fr kernels).
+// After the stream has synchronised: the MSM's phase times, and the call's device phases.
 static void das_collect_times(Engine& E, bool proofs, DasTimes* times) {
   if (proofs) {
     collect_msm_times(E);
@@ -447,10 +451,10 @@ static void das_collect_times(Engine& E, bool proofs, DasTimes* times) {
   }
   if (times) {
     *times = DasTimes();
-    cudaEventElapsedTime(&times->ms_fr, E.ev[7], E.ev[8]);
+    cudaEventElapsedTime(&times->ms_fr, E.caller_ev[DAS_START], E.caller_ev[DAS_FR_DONE]);
     if (proofs) {
-      cudaEventElapsedTime(&times->ms_msm, E.ev[8], E.ev[11]);
-      cudaEventElapsedTime(&times->ms_ecfft, E.ev[11], E.ev[12]);
+      cudaEventElapsedTime(&times->ms_msm, E.caller_ev[DAS_FR_DONE], E.caller_ev[DAS_MSM_DONE]);
+      cudaEventElapsedTime(&times->ms_ecfft, E.caller_ev[DAS_MSM_DONE], E.caller_ev[DAS_ECFFT_DONE]);
     }
   }
 }
@@ -468,14 +472,14 @@ void das_device(const void* d_tw, const DasBank* bank, const uint8_t* blobs, siz
   E.das_cells.ensure(bytes);
   const uint32_t* tw = (const uint32_t*)d_tw;
   B200_CUDA_CHECK(cudaMemcpyAsync(E.kzg_poly.ptr, blobs, bytes, cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[7], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[DAS_START], s));
   k_kzg_parse<<<(unsigned)((elems + 255) / 256), 256, 0, s>>>((uint32_t*)E.kzg_poly.ptr, elems);
   k_das_cells<<<(unsigned)n, DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((const uint32_t*)E.kzg_poly.ptr, tw, (uint32_t*)E.das_coefs.ptr,
                                                                   (uint32_t*)E.das_cells.ptr);
   if (bank) das_fk20(E, tw, *bank, n);
   else {
     B200_CUDA_CHECK(cudaGetLastError());
-    B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
+    B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[DAS_FR_DONE], s));
   }
   const size_t proof_bytes = bank ? n * DAS_CDS * DAS_XYZZ_BYTES : 0;
   E.ensure_host(bytes + proof_bytes);
@@ -507,7 +511,7 @@ void recover_device(const void* d_tw, const DasBank& bank, const uint8_t* ext, c
   const uint32_t* tw = (const uint32_t*)d_tw;
   B200_CUDA_CHECK(cudaMemcpyAsync(E.kzg_poly.ptr, ext, bytes, cudaMemcpyHostToDevice, s));
   B200_CUDA_CHECK(cudaMemcpyAsync(d_present, present, mask_bytes, cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[7], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[DAS_START], s));
   k_kzg_parse<<<(unsigned)((elems + 255) / 256), 256, 0, s>>>((uint32_t*)E.kzg_poly.ptr, elems);
   k_rec_vanishing<<<(unsigned)n, REC_Z, 0, s>>>(d_present, tw, d_z);
   k_rec_ifft<<<(unsigned)(2 * n), DAS_NTT_THREADS, DAS_NTT_SMEM, s>>>((uint32_t*)E.kzg_poly.ptr, d_z, tw);

@@ -187,11 +187,37 @@ __global__ void __launch_bounds__(DAS_L) k_ver_interp(const uint32_t* colres, si
   store_words(scalars + 8 * (M + M - DAS_L + j), s.neg());
 }
 
+// The verification drivers' marks in E.caller_ev
+enum VerifyMark { VERIFY_DECODE_START, VERIFY_DECODE_DONE, VERIFY_PARSE_START, VERIFY_PARSE_DONE, VERIFY_FR_START, VERIFY_FR_DONE };
+
+// Step 1 of both drivers: the npts points up into ver_in, k_ver_decode into ver_pts between the decode marks, and the statuses queued
+// back to E.h_result. The driver queues its own work behind it and synchronises.
+static void ver_decode(Engine& E, const VerifyPoint* points, size_t npts, uint8_t* d_status) {
+  cudaStream_t s = E.compute();
+  B200_CUDA_CHECK(cudaMemcpyAsync(E.ver_in.ptr, points, npts * sizeof(VerifyPoint), cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[VERIFY_DECODE_START], s));
+  k_ver_decode<<<(unsigned)((npts + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>((const VerifyPoint*)E.ver_in.ptr, npts,
+                                                                                           (uint32_t*)E.ver_pts.ptr, d_status);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[VERIFY_DECODE_DONE], s));
+  E.ensure_host(npts);
+  B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, d_status, npts, cudaMemcpyDeviceToHost, s));
+}
+
+// Step 3 of both drivers: the bank of 2 MSMs of M terms over the decoded points (one shared set), the scalars in sc, into out[0..1];
+// its time is ms_msm.
+static void ver_bank(Engine& E, const uint32_t* sc, size_t M, host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times) {
+  MsmJob job(sc, E.ver_pts.ptr, M, /*fr_mont=*/true);
+  job.batch = 2;
+  job.dest = MsmJob::HOST_ARRAY; job.out = out;
+  msm_device<Bls12381G1>(E, job);
+  thread_stats() = E.stats;
+  if (times) times->ms_msm = E.collect_timing ? E.stats.ms_total : 0.f;
+}
+
 int verify_device(const void* d_tw, const void* d_mono, const VerifyBatch& vb, const std::function<void()>& overlap,
                   const std::function<int(const uint8_t*)>& decide, const std::function<void(uint64_t*)>& challenge,
                   host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times) {
-  using C = Bls12381G1;
-  using HP = host::HXyzz<typename C::H>;
   EngineLease lease = acquire_engine();
   Engine& E = *lease.e;
   cudaStream_t s = E.compute();
@@ -222,21 +248,14 @@ int verify_device(const void* d_tw, const void* d_mono, const VerifyBatch& vb, c
   uint32_t* d_colres = d_rp + 8 * n;
 
   // 1. decode (and the cells behind it), statuses back; the host checks the cells and hashes meanwhile
-  B200_CUDA_CHECK(cudaMemcpyAsync(base, vb.points, in_bytes, cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[7], s));
-  k_ver_decode<<<(unsigned)((npts + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>((const VerifyPoint*)base, npts,
-                                                                                           (uint32_t*)E.ver_pts.ptr, d_status);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
-  E.ensure_host(npts);
-  B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, d_status, npts, cudaMemcpyDeviceToHost, s));
+  ver_decode(E, vb.points, npts, d_status);
   B200_CUDA_CHECK(cudaMemcpyAsync(d_cells, vb.cells, cell_bytes, cudaMemcpyHostToDevice, s));
   B200_CUDA_CHECK(cudaMemcpyAsync(d_idx, vb.index_words, idx_words * 4, cudaMemcpyHostToDevice, s));
   overlap();
   B200_CUDA_CHECK(cudaStreamSynchronize(s));
   if (times) {
     *times = VerifyTimes();
-    cudaEventElapsedTime(&times->ms_decode, E.ev[7], E.ev[8]);
+    cudaEventElapsedTime(&times->ms_decode, E.caller_ev[VERIFY_DECODE_START], E.caller_ev[VERIFY_DECODE_DONE]);
   }
   const int st = decide((const uint8_t*)E.h_result);
   if (st != 0) return st;
@@ -247,7 +266,7 @@ int verify_device(const void* d_tw, const void* d_mono, const VerifyBatch& vb, c
   B200_CUDA_CHECK(cudaMemcpyAsync(d_r, r, 32, cudaMemcpyHostToDevice, s));
   E.d_scalars.ensure(2 * M * 32 + 16);
   uint32_t* sc = (uint32_t*)E.d_scalars.ptr;
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[11], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[VERIFY_FR_START], s));
   k_kzg_parse<<<(unsigned)((n * DAS_L + 255) / 256), 256, 0, s>>>(d_cells, n * DAS_L);
   k_ver_powers<<<(unsigned)((n + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>(d_r, n, d_rp);
   k_ver_scalars<<<(unsigned)((M + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>(d_rp, d_cols, d_com_start, d_com_list, tw, n, U, sc);
@@ -255,19 +274,11 @@ int verify_device(const void* d_tw, const void* d_mono, const VerifyBatch& vb, c
   k_ver_interp<<<1, DAS_L, 0, s>>>(d_colres, used, M, sc);
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaMemcpyAsync((char*)E.ver_pts.ptr + npts * AFF, d_mono, DAS_L * AFF, cudaMemcpyDeviceToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[12], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[VERIFY_FR_DONE], s));
 
   // 3. the bank of 2 MSMs over the shared point set
-  E.stats.ms_h2d = 0;
-  HP res[2] = {HP::inf(), HP::inf()};
-  msm_device<C>(E, sc, E.ver_pts.ptr, M, /*fr_mont=*/true, 0, 0, -1, nullptr, 0, /*batch=*/2, /*point_sets=*/1, res);
-  thread_stats() = E.stats;
-  out[0] = res[0];
-  out[1] = res[1];
-  if (times) {
-    cudaEventElapsedTime(&times->ms_fr, E.ev[11], E.ev[12]);
-    times->ms_msm = E.collect_timing ? E.stats.ms_total : 0.f;
-  }
+  ver_bank(E, sc, M, out, times);
+  if (times) cudaEventElapsedTime(&times->ms_fr, E.caller_ev[VERIFY_FR_START], E.caller_ev[VERIFY_FR_DONE]);
   return 0;
 }
 
@@ -372,8 +383,6 @@ __global__ void __launch_bounds__(KZG_THREADS) k_kzg_ver_scalars(const uint32_t*
 int verify_blob_device(const void* d_roots, const BlobVerifyBatch& vb, const std::function<void()>& overlap,
                        const std::function<int(const uint8_t*)>& decide, const OpeningArgs* args, const uint64_t* r_mont,
                        host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times) {
-  using C = Bls12381G1;
-  using HP = host::HXyzz<typename C::H>;
   EngineLease lease = acquire_engine();
   Engine& E = *lease.e;
   cudaStream_t s = E.compute();
@@ -397,26 +406,19 @@ int verify_blob_device(const void* d_roots, const BlobVerifyBatch& vb, const std
   uint32_t* d_poly = (uint32_t*)E.kzg_poly.ptr;
 
   // 1. decode, statuses back, the blobs up and parsed behind them; the host checks the blobs and hashes meanwhile
-  B200_CUDA_CHECK(cudaMemcpyAsync(base, vb.points, in_bytes, cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[7], s));
-  k_ver_decode<<<(unsigned)((M + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>((const VerifyPoint*)base, M,
-                                                                                        (uint32_t*)E.ver_pts.ptr, d_status);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[8], s));
-  E.ensure_host(M);
-  B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, d_status, M, cudaMemcpyDeviceToHost, s));
+  ver_decode(E, vb.points, M, d_status);
   B200_CUDA_CHECK(cudaMemcpyAsync(d_poly, vb.blobs, elems * 32, cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[9], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[VERIFY_PARSE_START], s));
   k_kzg_parse<<<(unsigned)((elems + 255) / 256), 256, 0, s>>>(d_poly, elems);   // an element >= r is refused below; no use is made of it
   B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[10], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[VERIFY_PARSE_DONE], s));
   overlap();
   B200_CUDA_CHECK(cudaStreamSynchronize(s));
   float ms_parse = 0;
   if (times) {
     *times = VerifyTimes();
-    cudaEventElapsedTime(&times->ms_decode, E.ev[7], E.ev[8]);
-    cudaEventElapsedTime(&ms_parse, E.ev[9], E.ev[10]);
+    cudaEventElapsedTime(&times->ms_decode, E.caller_ev[VERIFY_DECODE_START], E.caller_ev[VERIFY_DECODE_DONE]);
+    cudaEventElapsedTime(&ms_parse, E.caller_ev[VERIFY_PARSE_START], E.caller_ev[VERIFY_PARSE_DONE]);
   }
   const int st = decide((const uint8_t*)E.h_result);
   if (st != 0) return st;
@@ -426,24 +428,18 @@ int verify_blob_device(const void* d_roots, const BlobVerifyBatch& vb, const std
   B200_CUDA_CHECK(cudaMemcpyAsync(d_r, r_mont, 32, cudaMemcpyHostToDevice, s));
   E.d_scalars.ensure(2 * M * 32 + 16);
   uint32_t* sc = (uint32_t*)E.d_scalars.ptr;
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[11], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[VERIFY_FR_START], s));
   k_ver_powers<<<(unsigned)((n + VER_THREADS - 1) / VER_THREADS), VER_THREADS, 0, s>>>(d_r, n, d_rp);
   k_kzg_eval<<<(unsigned)n, KZG_THREADS, 0, s>>>(d_poly, (const uint32_t*)d_roots, d_args, d_y);
   k_kzg_ver_scalars<<<1, KZG_THREADS, 0, s>>>(d_rp, d_args, d_y, n, sc);
   B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(E.ev[12], s));
+  B200_CUDA_CHECK(cudaEventRecord(E.caller_ev[VERIFY_FR_DONE], s));
 
   // 3. the bank of 2 MSMs over the decoded points
-  E.stats.ms_h2d = 0;
-  HP res[2] = {HP::inf(), HP::inf()};
-  msm_device<C>(E, sc, E.ver_pts.ptr, M, /*fr_mont=*/true, 0, 0, -1, nullptr, 0, /*batch=*/2, /*point_sets=*/1, res);
-  thread_stats() = E.stats;
-  out[0] = res[0];
-  out[1] = res[1];
+  ver_bank(E, sc, M, out, times);
   if (times) {
-    cudaEventElapsedTime(&times->ms_fr, E.ev[11], E.ev[12]);
+    cudaEventElapsedTime(&times->ms_fr, E.caller_ev[VERIFY_FR_START], E.caller_ev[VERIFY_FR_DONE]);
     times->ms_fr += ms_parse;
-    times->ms_msm = E.collect_timing ? E.stats.ms_total : 0.f;
   }
   return 0;
 }
