@@ -157,6 +157,8 @@ def load():
     lib.ctt_b200_eth_bls_last_timing.restype = None
     lib.ctt_b200_test_hash_to_g2.argtypes = [vp, sz, vp, sz, vp]
     lib.ctt_b200_test_hash_to_g2.restype = ci
+    lib.ctt_b200_test_map_to_g2.argtypes = [vp, sz, vp]
+    lib.ctt_b200_test_map_to_g2.restype = ci
     lib.ctt_b200_test_pairing.argtypes = [vp, vp, sz, vp]
     lib.ctt_b200_test_pairing.restype = ci
     lib.ctt_threadpool_new.argtypes = [ci]

@@ -328,6 +328,24 @@ int ctt_b200_test_hash_to_g2(const unsigned char* msg, size_t msg_len, const uns
   return 0;
 }
 
+int ctt_b200_test_map_to_g2(const void* uniform, size_t n, void* out_aff) {
+  if (n == 0) return 0;
+  EngineLease lease = acquire_engine();
+  Engine& E = *lease.e;
+  cudaStream_t s = E.compute();
+  void *d_uni, *d_out;
+  B200_CUDA_CHECK(cudaMalloc(&d_uni, n * ethbls::UNIFORM_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_out, n * ethbls::SIG_BYTES + 16));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_uni, uniform, n * ethbls::UNIFORM_BYTES, cudaMemcpyHostToDevice, s));
+  bls::k_bls_hash_to_g2<<<(unsigned)((n + bls::H2C_THREADS - 1) / bls::H2C_THREADS), bls::H2C_THREADS, 0, s>>>((const uint8_t*)d_uni, n,
+                                                                                                          (uint32_t*)d_out);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpyAsync(out_aff, d_out, n * ethbls::SIG_BYTES, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  cudaFree(d_uni); cudaFree(d_out);
+  return 0;
+}
+
 int ctt_b200_test_pairing(const void* g1_aff, const void* g2_aff, size_t n, void* gt_out) {
   if (n == 0) return -1;
   ethbls::pairing_device((const uint8_t*)g1_aff, nullptr, 0, (const uint8_t*)g2_aff, n, nullptr, (uint8_t*)gt_out, nullptr);

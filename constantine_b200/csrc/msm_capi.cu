@@ -9,8 +9,9 @@
 namespace b200 {
 B200_DECLARE_CURVE(Bls12381G1) B200_DECLARE_CURVE(Bn254G1) B200_DECLARE_CURVE(PallasEc) B200_DECLARE_CURVE(VestaEc)
 B200_DECLARE_CURVE(Bls12381G2) B200_DECLARE_CURVE(Bn254G2)
-B200_DECLARE_FIELD(Bls12381Fp) B200_DECLARE_FIELD(Bn254SnarksFp) B200_DECLARE_FIELD(PallasFp) B200_DECLARE_FIELD(VestaFp)
-B200_DECLARE_FIELD(Bls12381Fr) B200_DECLARE_FIELD(Bn254SnarksFr) B200_DECLARE_FIELD(PallasFr) B200_DECLARE_FIELD(VestaFr)
+B200_DECLARE_FIELD(Bls12381Fp, 1) B200_DECLARE_FIELD(Bn254SnarksFp, 1) B200_DECLARE_FIELD(PallasFp, 1) B200_DECLARE_FIELD(VestaFp, 1)
+B200_DECLARE_FIELD(Bls12381Fr, 1) B200_DECLARE_FIELD(Bn254SnarksFr, 1) B200_DECLARE_FIELD(PallasFr, 1) B200_DECLARE_FIELD(VestaFr, 1)
+B200_DECLARE_FIELD(Bls12381Fp, 2) B200_DECLARE_FIELD(Bn254SnarksFp, 2)
 
 struct Bases {
   int curve_id;
@@ -300,14 +301,16 @@ int ctt_b200_sm_count(void) {
 
 int ctt_b200_test_field_op(int field_id, int op, void* r, const void* a, const void* b, size_t count) {
   switch (field_id) {
-    case 0: return run_test_field_op<Bls12381Fp>(op, r, a, b, count);
-    case 1: return run_test_field_op<Bn254SnarksFp>(op, r, a, b, count);
-    case 2: return run_test_field_op<PallasFp>(op, r, a, b, count);
-    case 3: return run_test_field_op<VestaFp>(op, r, a, b, count);
-    case 4: return run_test_field_op<Bls12381Fr>(op, r, a, b, count);
-    case 5: return run_test_field_op<Bn254SnarksFr>(op, r, a, b, count);
-    case 6: return run_test_field_op<PallasFr>(op, r, a, b, count);
-    case 7: return run_test_field_op<VestaFr>(op, r, a, b, count);
+    case 0: return run_test_field_op<Bls12381Fp, 1>(op, r, a, b, count);
+    case 1: return run_test_field_op<Bn254SnarksFp, 1>(op, r, a, b, count);
+    case 2: return run_test_field_op<PallasFp, 1>(op, r, a, b, count);
+    case 3: return run_test_field_op<VestaFp, 1>(op, r, a, b, count);
+    case 4: return run_test_field_op<Bls12381Fr, 1>(op, r, a, b, count);
+    case 5: return run_test_field_op<Bn254SnarksFr, 1>(op, r, a, b, count);
+    case 6: return run_test_field_op<PallasFr, 1>(op, r, a, b, count);
+    case 7: return run_test_field_op<VestaFr, 1>(op, r, a, b, count);
+    case 8: return run_test_field_op<Bls12381Fp, 2>(op, r, a, b, count);
+    case 9: return run_test_field_op<Bn254SnarksFp, 2>(op, r, a, b, count);
   }
   return -1;
 }

@@ -1,15 +1,18 @@
 // Test hooks, the on-device input generator and the host-side partial-sum combiner (templated bodies).
 #pragma once
+#include <type_traits>
 #include "msm_engine.cuh"
 
 namespace b200 {
 
 // ---- test kernels -------------------------------------------------------------------------------------------
-template <class F>
+constexpr int TEST_FIELD_OPS = 15;   // op codes 0 .. TEST_FIELD_OPS - 1 of k_test_field_op
+
+// T = Fp<F> or Fp2<F>; op 11 (the paired out-of-line multiplier) exists for Fp only
+template <class T>
 __global__ void k_test_field_op(int op, uint32_t* r, const uint32_t* a, const uint32_t* b, size_t count) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
-  using T = Fp<F>;
   T x, y, z;
   load_words(x, a + i * T::WORDS);
   load_words(y, b + i * T::WORDS);
@@ -18,10 +21,22 @@ __global__ void k_test_field_op(int op, uint32_t* r, const uint32_t* a, const ui
     case 1: z = x + y; break;
     case 2: z = x - y; break;
     case 3: z = x.neg(); break;
+    case 4: z = x.dbl(); break;
     case 5: z = T::dot2_u(x, y, x + y, x - y); break;   // x y + (x + y)(x - y), one reduction
     case 6: z = x.sqr_u() + y.sqr_u(); break;           // dedicated squaring
     case 7: z = fe_inverse(x) * x; break;                // safegcd inverse (field_inv.cuh): must give one, or zero for x = 0
-    default: z = x.dbl(); break;
+    case 8: z = fe_inverse(x); break;                    // the inverse itself, so a non-canonical result shows
+    case 9: z = x.inv(); break;                          // Fermat inverse (generator hook, precomputed tables)
+    case 10: z = x.mul_u(y); break;                      // inline unrolled multiplier (op 0 is the out-of-line one for 12 limbs)
+    case 11:
+      if constexpr (std::is_same<T, Fp<typename T::Params>>::value) {
+        const typename T::Pair q = T::mul2_call(x, y, x + y, x - y);
+        z = q.a + q.b;
+      }
+      break;
+    case 12: z = x; z.cneg(y.word(0) & 1u); break;
+    case 13: z = x.sqr(); break;
+    case 14: z = T::dot2_u(x, y, y, x); break;          // 2 x y, four free operands: x = y = p - 1 is the 3p worst case
   }
   store_words(r + i * T::WORDS, z);
 }
@@ -47,16 +62,19 @@ __global__ void k_test_ec_op(int op, uint32_t* r, const uint32_t* p, const uint3
   store_xyzz(r, i, R);
 }
 
-template <class F>
+// DEG = 1: elements of Fp<F>; DEG = 2: elements of Fp2<F>, c0 then c1 (the layout of G2 coordinates in the ABI)
+template <class F, int DEG>
 int run_test_field_op(int op, void* r, const void* a, const void* b, size_t count) {
+  using T = typename std::conditional<DEG == 2, Fp2<F>, Fp<F>>::type;
+  if (op < 0 || op >= TEST_FIELD_OPS || (DEG == 2 && op == 11)) return -1;
   EngineLease lease = acquire_engine();
   Engine& E = *lease.e;
-  size_t bytes = count * F::N64 * 8;
+  size_t bytes = count * DEG * F::N64 * 8;
   void *da, *db, *dr;
   B200_CUDA_CHECK(cudaMalloc(&da, bytes + 16)); B200_CUDA_CHECK(cudaMalloc(&db, bytes + 16)); B200_CUDA_CHECK(cudaMalloc(&dr, bytes + 16));
   B200_CUDA_CHECK(cudaMemcpyAsync(da, a, bytes, cudaMemcpyHostToDevice, E.stream));
   B200_CUDA_CHECK(cudaMemcpyAsync(db, b, bytes, cudaMemcpyHostToDevice, E.stream));
-  k_test_field_op<F><<<(unsigned)((count + 127) / 128), 128, 0, E.stream>>>(op, (uint32_t*)dr, (const uint32_t*)da, (const uint32_t*)db, count);
+  k_test_field_op<T><<<(unsigned)((count + 127) / 128), 128, 0, E.stream>>>(op, (uint32_t*)dr, (const uint32_t*)da, (const uint32_t*)db, count);
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaStreamSynchronize(E.stream));
   B200_CUDA_CHECK(cudaMemcpyAsync(r, dr, bytes, cudaMemcpyDeviceToHost, E.stream));
@@ -222,7 +240,7 @@ void* run_precompute_table(const void* d_points, size_t n, int c, int* W_out) {
   extern template int run_test_ec_op<DESC>(int, void*, const void*, const void*, size_t);                         \
   extern template int run_sum_partials<DESC>(int, void*, const void*, size_t);                                    \
   extern template int run_scalar_mul_u64<DESC>(const void*, const void*, size_t, void*);
-#define B200_INSTANTIATE_FIELD(F) template int run_test_field_op<F>(int, void*, const void*, const void*, size_t);
-#define B200_DECLARE_FIELD(F) extern template int run_test_field_op<F>(int, void*, const void*, const void*, size_t);
+#define B200_INSTANTIATE_FIELD(F, DEG) template int run_test_field_op<F, DEG>(int, void*, const void*, const void*, size_t);
+#define B200_DECLARE_FIELD(F, DEG) extern template int run_test_field_op<F, DEG>(int, void*, const void*, const void*, size_t);
 
 }  // namespace b200

@@ -243,9 +243,13 @@ def add_polys(f, g):
 
 
 def iso_apply(polys, pt):
+    """The isogeny at an affine point; None (the identity) where a denominator vanishes (RFC 9380 section 6.6.3)."""
     xn, xd, yn, yd = polys
     x, y = pt
-    return mul(p_eval(xn, x), inv(p_eval(xd, x))), mul(y, mul(p_eval(yn, x), inv(p_eval(yd, x))))
+    dx, dy = p_eval(xd, x), p_eval(yd, x)
+    if dx == ZERO or dy == ZERO:
+        return None
+    return mul(p_eval(xn, x), inv(dx)), mul(y, mul(p_eval(yn, x), inv(dy)))
 
 
 def iso_candidates():
