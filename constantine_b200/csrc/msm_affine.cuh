@@ -11,8 +11,10 @@
 //     trees is one dense array of independent pair additions, because every bucket's slots at every level are laid out by
 //     prefix sums of ceil(n_b / 2^r) (k_level_blocksums / k_level_scan / k_level_offsets): slot j of bucket b at level r+1 is the
 //     sum of slots 2j and 2j+1 of level r. No collisions exist by construction, nothing is queued or rescheduled.
-//   * k_affine_plan (one thread per sorted entry) writes, for every level, the source of each slot -- so the arithmetic kernel
-//     k_affine_pairs is a plain list processor: lane = slot, perfectly regular, independent of the digit distribution.
+//   * k_affine_plan (one thread per sorted entry) writes, for every level, the source of each slot -- so the arithmetic kernels
+//     k_affine_pairs / k_affine_pairs_ws are plain list processors: lane = slot, perfectly regular, independent of the digit
+//     distribution. Both take their slots from PairSlots and do the arithmetic of a slot in pair_factor (pass 1) and
+//     pair_result (pass 2); they differ only in where the operands come from.
 //   * the shared inversion is PER THREAD: a thread walks M slots (M = level size / resident threads, ~150 at N = 2^20),
 //     multiplies their denominators into a running product (prefix products parked in a coalesced global scratch), inverts
 //     once (safegcd, field_inv.cuh) and unwinds: 1 + 5 multiplications per addition + inversion / M. Lanes never wait for
@@ -325,17 +327,19 @@ B200_DEV T load_x(const uint32_t* src, uint32_t ref) {
   else load_words_rw(x, src + (size_t)ref * (2 * T::WORDS));
   return x;
 }
+// the ordinate of an operand as loaded -> as added: at level 0 the plan reference carries the sign in bit 31. zero: y = 0, which with
+// x = 0 marks the point at infinity (stored as (0, 0)).
 template <class T, bool FIRST>
-B200_DEV T load_y(const uint32_t* src, uint32_t ref, bool& is_inf_if_x_zero) {
+B200_DEV void decode_y(T& y, uint32_t ref, bool& zero) {
+  zero = y.is_zero();
+  if constexpr (FIRST) y.cneg((ref >> 31) != 0);
+}
+template <class T, bool FIRST>
+B200_DEV T load_y(const uint32_t* src, uint32_t ref, bool& zero) {
   T y;
-  if constexpr (FIRST) {
-    load_words(y, src + (size_t)(ref & 0x7FFFFFFFu) * (2 * T::WORDS) + T::WORDS);
-    is_inf_if_x_zero = y.is_zero();
-    y.cneg((ref >> 31) != 0);
-  } else {
-    load_words_rw(y, src + (size_t)ref * (2 * T::WORDS) + T::WORDS);
-    is_inf_if_x_zero = y.is_zero();
-  }
+  if constexpr (FIRST) load_words(y, src + (size_t)(ref & 0x7FFFFFFFu) * (2 * T::WORDS) + T::WORDS);
+  else load_words_rw(y, src + (size_t)ref * (2 * T::WORDS) + T::WORDS);
+  decode_y<T, FIRST>(y, ref, zero);
   return y;
 }
 
@@ -350,6 +354,50 @@ B200_DEV int classify_pair(bool single, const T& x1, const T& y1, bool inf1, con
   if (!(y1 == y2) || y1.is_zero()) return PAIR_INF;     // P + (-P), or doubling a point of order two
   den = y1.dbl();
   return PAIR_DBL;
+}
+
+// The slot arithmetic of both pair kernels, which differ only in where the operands come from.
+// Pass 1 of slot (a, b): multiplies its factor, if it has one, into the running product, from the abscissae as loaded.
+template <class T, bool FIRST>
+B200_DEV void pair_factor(const uint32_t* src, uint32_t a, uint32_t b, const T& x1, const T& x2, T& run) {
+  const bool single = b == AFF_NONE;
+  T den = x2 - x1;
+  bool contributes = !single;
+  if (!single && (den.is_zero() || x1.is_zero() || x2.is_zero())) {
+    // rare: equal abscissae (doubling or cancellation) or a possible infinity operand -- needs the ordinates
+    bool z1, z2;
+    const T y1 = load_y<T, FIRST>(src, a, z1), y2 = load_y<T, FIRST>(src, b, z2);
+    const int kind = classify_pair(false, x1, y1, z1 && x1.is_zero(), x2, y2, z2 && x2.is_zero(), den);
+    contributes = kind >= PAIR_ADD;
+  }
+  if (contributes) run = run.mul_u(den);
+}
+
+// Pass 2 of slot j: R = P1 + P2 from the decoded operands and their y = 0 flags (P2 unused when single). inv is the inverse of
+// the running product up to slot j and moves past it; prefix() returns the running product before slot j, and is called only
+// for an addition or a doubling of a slot j > 0.
+template <class T, class Prefix>
+B200_DEV Aff<T> pair_result(const Aff<T>& P1, bool z1, const Aff<T>& P2, bool z2, bool single, uint32_t j, T& inv, Prefix prefix) {
+  T den;
+  const int kind = classify_pair(single, P1.x, P1.y, z1 && P1.x.is_zero(), P2.x, P2.y, z2 && P2.x.is_zero(), den);
+  Aff<T> R;
+  if (kind < PAIR_ADD) {
+    if (kind == PAIR_COPY1) R = P1;
+    else if (kind == PAIR_COPY2) R = P2;
+    else { R.x = T::zero(); R.y = T::zero(); }
+  } else {
+    T inv_den = inv;
+    if (j > 0) inv_den = inv.mul_u(prefix());
+    inv = inv.mul_u(den);
+    T num;
+    if (kind == PAIR_ADD) num = P2.y - P1.y;
+    else { const T xx = P1.x.sqr(); num = xx.dbl() + xx; }     // 3 x^2 (a = 0); rare: rolled multiplier
+    // unrolled multipliers: the rolled form spends a large share of its issue slots rotating registers
+    const T lam = num.mul_u(inv_den);
+    R.x = lam.sqr_u() - P1.x - P2.x;
+    R.y = lam.mul_u(P1.x - R.x) - P1.y;
+  }
+  return R;
 }
 
 #ifndef B200_AFF_THREADS
@@ -371,38 +419,53 @@ B200_DEV void prefetch_point(const uint32_t* src, uint32_t ref) {
   prefetch_span(src + (size_t)idx * (2 * T::WORDS), 2 * T::WORDS * 4);
 }
 
-// dst[p] = src[a_p] (+ src[b_p]) for p < *total_ptr. Persistent: the grid's threads split the slots evenly; a warp owns a
+// Slots, and rows of the prefix-product scratch, per slot-owning thread for a level of `slots` slots.
+__host__ __device__ __forceinline__ size_t pair_rows(size_t slots, size_t threads) { return (slots + threads - 1) / threads; }
+
+// The slot schedule of a pair-kernel launch. The `threads` slot-owning threads of the grid split the slots evenly: a warp owns a
 // contiguous range of 32 M slots and lane l takes slots l, l + 32, ... of it (coalesced plans, outputs and level >= 1 operands).
+// perm / range (level 0 of a host call whose points arrive in pieces): the launch handles the slots perm[range[0] .. range[1]),
+// i.e. the pairs whose operands all lie in the pieces that have arrived; otherwise slots 0 .. *total_ptr in order.
+// tid: index of a thread among the slot-owning threads.
+struct PairSlots {
+  const uint32_t* perm;
+  uint32_t total, M;
+  B200_DEV PairSlots(const uint32_t* total_ptr, const uint32_t* perm_, const uint32_t* range, size_t threads) {
+    const uint32_t range_begin = range ? range[0] : 0u;
+    total = range ? range[1] - range[0] : *total_ptr;
+    perm = perm_;
+    if (perm) perm += range_begin;
+    M = (uint32_t)pair_rows(total, threads);
+  }
+  B200_DEV size_t first(size_t tid) const { return (tid & ~(size_t)31) * M + (tid & 31u); }
+  // slots of the thread: first + 32 j for j < count
+  B200_DEV uint32_t count(size_t tid) const {
+    const size_t f = first(tid);
+    if (f >= total) return 0u;
+    const uint32_t c = (uint32_t)(((size_t)total - f + 31) / 32);
+    return c < M ? c : M;
+  }
+  B200_DEV size_t slot(size_t tid, uint32_t j) const {
+    const size_t t = first(tid) + 32u * (size_t)j;
+    return perm ? (size_t)perm[t] : t;
+  }
+};
+
+// dst[p] = src[a_p] (+ src[b_p]) for the slots p of PairSlots. Persistent: every thread owns slots.
 template <class T, bool FIRST>
 __global__ void __launch_bounds__(B200_AFF_THREADS, (T::WORDS <= 12) ? B200_AFF_MIN_BLOCKS : 1)
 k_affine_pairs(const void* __restrict__ plan, const uint32_t* __restrict__ total_ptr, const uint32_t* src, uint32_t* dst, uint4* scratch,
                const uint32_t* __restrict__ perm = nullptr, const uint32_t* __restrict__ range = nullptr) {
-  // perm / range (level 0 of a host call whose points arrive in chunks): this launch handles the slots perm[range[0] .. range[1]),
-  // i.e. the pairs whose operands all lie in the chunks that have arrived; otherwise slots 0 .. *total_ptr in order.
   const size_t threads = (size_t)gridDim.x * blockDim.x;
   const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t range_begin = range ? range[0] : 0u;
-  const uint32_t total = range ? range[1] - range[0] : *total_ptr;
-  if (perm) perm += range_begin;
-  const uint32_t M = (uint32_t)(((size_t)total + threads - 1) / threads);
+  const PairSlots S(total_ptr, perm, range, threads);
   const unsigned lane = threadIdx.x & 31u;
-  const size_t warp_base = (tid - lane) * (size_t)M;          // first slot of this warp
-  if (warp_base >= total) return;
-  // slots of this lane: warp_base + lane + 32 j, j < cnt
-  uint32_t cnt = 0;
-  {
-    const size_t first = warp_base + lane;
-    if (first < total) {
-      const size_t left = (size_t)total - first;
-      cnt = (uint32_t)((left + 31) / 32);
-      if (cnt > M) cnt = M;
-    }
-  }
+  if (S.count(tid - lane) == 0) return;      // no slot for this warp
+  const uint32_t cnt = S.count(tid);
   // ---- pass 1: running product of the denominators; prefix products to the scratch
   T run = T::one();
   {
-    auto slot_of = [&](size_t t) -> size_t { return perm ? (size_t)perm[t] : t; };
-    PairTask t_next = cnt ? load_task<FIRST>(plan, slot_of(warp_base + lane)) : PairTask{0u, AFF_NONE};
+    PairTask t_next = cnt ? load_task<FIRST>(plan, S.slot(tid, 0)) : PairTask{0u, AFF_NONE};
     T x1n = T::zero(), x2n = T::zero();
     if (cnt) {
       x1n = load_x<T, FIRST>(src, t_next.a);
@@ -413,21 +476,11 @@ k_affine_pairs(const void* __restrict__ plan, const uint32_t* __restrict__ total
       const PairTask t = t_next;
       const T x1 = x1n, x2 = x2n;
       if (j + 1 < cnt) {
-        t_next = load_task<FIRST>(plan, slot_of(warp_base + lane + 32u * (size_t)(j + 1)));
+        t_next = load_task<FIRST>(plan, S.slot(tid, j + 1));
         x1n = load_x<T, FIRST>(src, t_next.a);
         if (t_next.b != AFF_NONE) x2n = load_x<T, FIRST>(src, t_next.b);
       }
-      const bool single = t.b == AFF_NONE;
-      T den = x2 - x1;
-      bool contributes = !single;
-      if (!single && (den.is_zero() || x1.is_zero() || x2.is_zero())) {
-        // rare: equal abscissae (doubling or cancellation) or a possible infinity operand -- needs the ordinates
-        bool z1, z2;
-        const T y1 = load_y<T, FIRST>(src, t.a, z1), y2 = load_y<T, FIRST>(src, t.b, z2);
-        const int kind = classify_pair(false, x1, y1, z1 && x1.is_zero(), x2, y2, z2 && x2.is_zero(), den);
-        contributes = kind >= PAIR_ADD;
-      }
-      if (contributes) run = run.mul_u(den);
+      pair_factor<T, FIRST>(src, t.a, t.b, x1, x2, run);
       scratch_store(scratch, threads, tid, j, run);
     }
   }
@@ -435,8 +488,7 @@ k_affine_pairs(const void* __restrict__ plan, const uint32_t* __restrict__ total
   T inv = fe_inverse(run);
   // ---- pass 2: unwind, last slot first. The operands of slot j - 1 (found through its plan entry) and the prefix product it
   // will need are pulled into L2 while slot j is being computed: the dependent plan -> point gather then costs an L2 hit.
-  auto slot_of2 = [&](size_t t) -> size_t { return perm ? (size_t)perm[t] : t; };
-  size_t p_prev = cnt ? slot_of2(warp_base + lane + 32u * (size_t)(cnt - 1)) : 0;
+  size_t p_prev = cnt ? S.slot(tid, cnt - 1) : 0;
   PairTask t_prev = cnt ? load_task<FIRST>(plan, p_prev) : PairTask{0u, AFF_NONE};
 #pragma unroll 1
   for (uint32_t jj = cnt; jj > 0; jj--) {
@@ -444,7 +496,7 @@ k_affine_pairs(const void* __restrict__ plan, const uint32_t* __restrict__ total
     const size_t p = p_prev;
     const PairTask t = t_prev;
     if (j > 0) {
-      p_prev = slot_of2(warp_base + lane + 32u * (size_t)(j - 1));
+      p_prev = S.slot(tid, j - 1);
       t_prev = load_task<FIRST>(plan, p_prev);
       prefetch_point<T, FIRST>(src, t_prev.a);
       if (t_prev.b != AFF_NONE) prefetch_point<T, FIRST>(src, t_prev.b);
@@ -465,33 +517,14 @@ k_affine_pairs(const void* __restrict__ plan, const uint32_t* __restrict__ total
     } else {
       P2.x = T::zero(); P2.y = T::zero();
     }
-    T den;
-    const int kind = classify_pair(single, P1.x, P1.y, z1 && P1.x.is_zero(), P2.x, P2.y, z2 && P2.x.is_zero(), den);
-    Aff<T> R;
-    if (kind < PAIR_ADD) {
-      if (kind == PAIR_COPY1) R = P1;
-      else if (kind == PAIR_COPY2) R = P2;
-      else { R.x = T::zero(); R.y = T::zero(); }
-    } else {
-      T inv_den = inv;
-      if (j > 0) inv_den = inv.mul_u(scratch_load<T>(scratch, threads, tid, j - 1));
-      inv = inv.mul_u(den);
-      T num;
-      if (kind == PAIR_ADD) num = P2.y - P1.y;
-      else { const T xx = P1.x.sqr(); num = xx.dbl() + xx; }     // 3 x^2 (a = 0); rare: rolled multiplier
-      // unrolled multipliers: the rolled form spends a large share of its issue slots rotating registers
-      const T lam = num.mul_u(inv_den);
-      R.x = lam.sqr_u() - P1.x - P2.x;
-      R.y = lam.mul_u(P1.x - R.x) - P1.y;
-    }
-    store_affine(dst, p, R);
+    store_affine(dst, p, pair_result(P1, z1, P2, z2, single, j, inv, [&] { return scratch_load<T>(scratch, threads, tid, j - 1); }));
   }
 }
 
 // ------------------------------------------------------------------------------------------------ warp-specialised pair kernel
-// Same slots, same per-thread batches, same arithmetic as k_affine_pairs (so the same results), but the operand gathers are moved
-// out of the threads that multiply. A block is AFF_WS_CONSUMERS consumer warps plus ONE producer warp. Consumer warp w owns the
-// slots k_affine_pairs would give a warp (a contiguous range of 32 M slots, lane l takes l, l + 32, ...). For every consumer warp,
+// The slot schedule (PairSlots, over the consumer threads) and the slot arithmetic (pair_factor, pair_result) of k_affine_pairs,
+// with the operand gathers moved out of the threads that multiply. A block is AFF_WS_CONSUMERS consumer warps plus ONE producer
+// warp. For every consumer warp,
 // in the order that warp consumes them, the producer reads the plan entry and issues cp.async copies of the operands into a ring of
 // stages in shared memory (pass 1: x1, x2; pass 2: P1, P2 and the slot's prefix product), then signals the stage's `full` mbarrier
 // (cp.async.mbarrier.arrive.noinc: the arrival lands when the copies have). A consumer waits on `full`, reads the stage into
@@ -570,22 +603,9 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
     }
   }
   __syncthreads();
-  // slots as in k_affine_pairs, over the consumer threads only
+  // the slots are those of the consumer threads only
   const size_t threads = (size_t)gridDim.x * NC * 32;
-  const uint32_t range_begin = range ? range[0] : 0u;
-  const uint32_t total = range ? range[1] - range[0] : *total_ptr;
-  if (perm) perm += range_begin;
-  const uint32_t M = (uint32_t)(((size_t)total + threads - 1) / threads);
-  auto count_of = [&](size_t tid) -> uint32_t {      // slots of consumer thread tid: warp_base + lane + 32 j, j < count
-    const size_t first = (tid & ~(size_t)31) * M + (tid & 31u);
-    if (first >= total) return 0u;
-    const uint32_t c = (uint32_t)(((size_t)total - first + 31) / 32);
-    return c < M ? c : M;
-  };
-  auto slot_at = [&](size_t tid, uint32_t j) -> size_t {
-    const size_t t = (tid & ~(size_t)31) * M + (tid & 31u) + 32u * (size_t)j;
-    return perm ? (size_t)perm[t] : t;
-  };
+  const PairSlots S(total_ptr, perm, range, threads);
   uint4* const ring_base = reinterpret_cast<uint4*>(aff_ring_raw);
 
   if (warp == NC) {
@@ -594,15 +614,15 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
 #pragma unroll
     for (int w = 0; w < NC; w++) {
       const size_t tid = ((size_t)blockIdx.x * NC + w) * 32 + lane;
-      n[w] = count_of(tid - lane);                   // iterations of warp w (lane 0 has the most slots)
-      cnt[w] = count_of(tid);
+      n[w] = S.count(tid - lane);                 // iterations of warp w (lane 0 has the most slots)
+      cnt[w] = S.count(tid);
     }
     auto tid_of = [&](int w) { return ((size_t)blockIdx.x * NC + w) * 32 + lane; };
     auto src_of = [&](uint32_t ref) { return src + (size_t)(FIRST ? (ref & 0x7FFFFFFFu) : ref) * (2 * T::WORDS); };
     // the plan entries of the next round are loaded while this round's copies are issued
     uint32_t ta[NC], tb[NC], tp[NC];
     auto fetch_task = [&](int w, uint32_t j) {
-      const size_t p = slot_at(tid_of(w), j);
+      const size_t p = S.slot(tid_of(w), j);
       const PairTask t = load_task<FIRST>(plan, p);
       ta[w] = t.a; tb[w] = t.b; tp[w] = (uint32_t)p;
     };
@@ -677,7 +697,7 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
 
   // ================= consumers
   const size_t tid = ((size_t)blockIdx.x * NC + warp) * 32 + lane;
-  const uint32_t n = count_of(tid - lane), cnt = count_of(tid);
+  const uint32_t n = S.count(tid - lane), cnt = S.count(tid);
   if (n == 0) return;
   const uint4* ring = ring_base + (size_t)warp * RG::ROWS * 32;
   // ---- pass 1: running product of the denominators; prefix products to the scratch
@@ -690,17 +710,7 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
     const T x1 = ring_load<T>(ring, s * 2 * V, lane), x2 = ring_load<T>(ring, s * 2 * V + V, lane);
     mbar_arrive(&empty1[warp][s]);
     if (j >= cnt) continue;
-    const bool single = b == AFF_NONE;
-    T den = x2 - x1;
-    bool contributes = !single;
-    if (!single && (den.is_zero() || x1.is_zero() || x2.is_zero())) {
-      // rare: equal abscissae (doubling or cancellation) or a possible infinity operand -- needs the ordinates
-      bool z1, z2;
-      const T y1 = load_y<T, FIRST>(src, a, z1), y2 = load_y<T, FIRST>(src, b, z2);
-      const int kind = classify_pair(false, x1, y1, z1 && x1.is_zero(), x2, y2, z2 && x2.is_zero(), den);
-      contributes = kind >= PAIR_ADD;
-    }
-    if (contributes) run = run.mul_u(den);
+    pair_factor<T, FIRST>(src, a, b, x1, x2, run);
     scratch_store(scratch, threads, tid, j, run);
   }
   mbar_arrive(&drained[warp]);      // release: the producer's pass-2 copies of the prefix products come after these stores
@@ -723,63 +733,47 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
     const T pre = ring_load<T>(ring, row + 4 * V, lane);
     mbar_arrive(&empty2[warp][s]);
     if (j >= cnt) continue;
-    const bool z1 = P1.y.is_zero(), z2 = P2.y.is_zero();
-    if constexpr (FIRST) {
-      P1.y.cneg((a >> 31) != 0);
-      if (!single) P2.y.cneg((b >> 31) != 0);
-    }
-    T den;
-    const int kind = classify_pair(single, P1.x, P1.y, z1 && P1.x.is_zero(), P2.x, P2.y, z2 && P2.x.is_zero(), den);
-    Aff<T> R;
-    if (kind < PAIR_ADD) {
-      if (kind == PAIR_COPY1) R = P1;
-      else if (kind == PAIR_COPY2) R = P2;
-      else { R.x = T::zero(); R.y = T::zero(); }
-    } else {
-      T inv_den = inv;
-      if (j > 0) inv_den = inv.mul_u(pre);
-      inv = inv.mul_u(den);
-      T num;
-      if (kind == PAIR_ADD) num = P2.y - P1.y;
-      else { const T xx = P1.x.sqr(); num = xx.dbl() + xx; }     // 3 x^2 (a = 0); rare: rolled multiplier
-      const T lam = num.mul_u(inv_den);
-      R.x = lam.sqr_u() - P1.x - P2.x;
-      R.y = lam.mul_u(P1.x - R.x) - P1.y;
-    }
-    store_affine(dst, p, R);
+    bool z1, z2 = false;
+    decode_y<T, FIRST>(P1.y, a, z1);
+    if (!single) decode_y<T, FIRST>(P2.y, b, z2);
+    store_affine(dst, p, pair_result(P1, z1, P2, z2, single, j, inv, [&] { return pre; }));
   }
 }
 
-// Pair kernel of a level: the warp-specialised one where its ring fits in shared memory, k_affine_pairs otherwise.
+// The pair kernel of a level: the warp-specialised one where its ring fits in shared memory, k_affine_pairs otherwise.
 template <class T>
-constexpr int affine_pairs_slot_threads() { return AffRing<T>::USED ? 32 * AFF_WS_CONSUMERS : B200_AFF_THREADS; }   // threads per block that own slots
+struct PairKernel {
+  static constexpr bool WS = AffRing<T>::USED;
+  static constexpr int THREADS = WS ? AFF_WS_THREADS : B200_AFF_THREADS;                 // per block
+  static constexpr int SLOT_THREADS = WS ? 32 * AFF_WS_CONSUMERS : B200_AFF_THREADS;     // per block, that own slots
+  static constexpr int SMEM = WS ? (int)AffRing<T>::BYTES : 0;                           // dynamic shared memory per block
+  template <bool FIRST>
+  static auto entry() {
+    if constexpr (WS) return k_affine_pairs_ws<T, FIRST>;
+    else return k_affine_pairs<T, FIRST>;
+  }
+};
 
 // resident blocks per SM of the pair kernel (also raises the dynamic shared-memory limit of the warp-specialised kernel)
 template <class T>
 cudaError_t affine_pairs_blocks_per_sm(int* bps) {
-  int b1 = 0, b2 = 0;
+  using K = PairKernel<T>;
+  int b[2] = {0, 0};
   cudaError_t e;
-  if constexpr (AffRing<T>::USED) {
-    constexpr int bytes = (int)AffRing<T>::BYTES;
-    if ((e = cudaFuncSetAttribute(k_affine_pairs_ws<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_affine_pairs_ws<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)) != cudaSuccess) return e;
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, k_affine_pairs_ws<T, true>, AFF_WS_THREADS, bytes)) != cudaSuccess) return e;
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, k_affine_pairs_ws<T, false>, AFF_WS_THREADS, bytes)) != cudaSuccess) return e;
-  } else {
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, k_affine_pairs<T, true>, B200_AFF_THREADS, 0)) != cudaSuccess) return e;
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, k_affine_pairs<T, false>, B200_AFF_THREADS, 0)) != cudaSuccess) return e;
+  for (int f = 0; f < 2; f++) {
+    const auto k = f == 0 ? K::template entry<true>() : K::template entry<false>();
+    if (K::SMEM && (e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM)) != cudaSuccess) return e;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b[f], k, K::THREADS, K::SMEM)) != cudaSuccess) return e;
   }
-  *bps = b2 < b1 ? b2 : b1;
+  *bps = b[1] < b[0] ? b[1] : b[0];
   return cudaSuccess;
 }
 
 template <class T, bool FIRST>
 void launch_affine_pairs(unsigned grid, cudaStream_t s, const void* plan, const uint32_t* total_ptr, const uint32_t* src, uint32_t* dst, uint4* scratch,
                          const uint32_t* perm = nullptr, const uint32_t* range = nullptr) {
-  if constexpr (AffRing<T>::USED)
-    k_affine_pairs_ws<T, FIRST><<<grid, AFF_WS_THREADS, AffRing<T>::BYTES, s>>>(plan, total_ptr, src, dst, scratch, perm, range);
-  else
-    k_affine_pairs<T, FIRST><<<grid, B200_AFF_THREADS, 0, s>>>(plan, total_ptr, src, dst, scratch, perm, range);
+  using K = PairKernel<T>;
+  K::template entry<FIRST>()<<<grid, K::THREADS, K::SMEM, s>>>(plan, total_ptr, src, dst, scratch, perm, range);
 }
 
 }  // namespace b200

@@ -564,9 +564,8 @@ void affine_levels(Engine& E, const MsmSizes& z, int AL, size_t entries, size_t 
     bps_cache[E.device] = bps;
   }
   const unsigned aff_grid = (unsigned)(E.sm_count * bps);
-  const size_t aff_threads = (size_t)aff_grid * affine_pairs_slot_threads<T>();
-  const size_t per_thread = (level_cap(1) + aff_threads - 1) / aff_threads;
-  E.aff_scratch.ensure(per_thread * aff_threads * (size_t)T::WORDS * 4);
+  const size_t aff_threads = (size_t)aff_grid * PairKernel<T>::SLOT_THREADS;
+  E.aff_scratch.ensure(pair_rows(level_cap(1), aff_threads) * aff_threads * (size_t)T::WORDS * 4);
   uint32_t* head = (uint32_t*)E.aff_head.ptr;
   uint32_t* tail = (uint32_t*)E.aff_tail.ptr;
   uint32_t* off = (uint32_t*)E.aff_off.ptr;
