@@ -155,6 +155,10 @@ def load():
     lib.ctt_b200_eth_bls_deserialize_signature_compressed.restype = ci
     lib.ctt_b200_eth_bls_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 6
     lib.ctt_b200_eth_bls_last_timing.restype = None
+    lib.ctt_b200_eth_bls_batch_verify_sets.argtypes = [vp, vp, vp, vp, vp, sz, vp, ctypes.POINTER(sz)]
+    lib.ctt_b200_eth_bls_batch_verify_sets.restype = ub
+    lib.ctt_b200_eth_bls_verify_sets.argtypes = [vp, vp, vp, vp, vp, sz, vp]
+    lib.ctt_b200_eth_bls_verify_sets.restype = ub
     lib.ctt_b200_test_hash_to_g2.argtypes = [vp, sz, vp, sz, vp]
     lib.ctt_b200_test_hash_to_g2.restype = ci
     lib.ctt_b200_test_map_to_g2.argtypes = [vp, sz, vp]

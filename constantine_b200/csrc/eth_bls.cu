@@ -10,18 +10,23 @@
 //   device (one engine lease and stream): hash to G2 (h2c_kernels.cuh), [r_i]PK_i (k_scalar_mul_u64 with a base per item), n + 1 Miller
 //           loops, their tree product and the final exponentiation (pairing_kernels.cuh); one flag comes back.
 // aggregate_verify of n pairs (PK_i, m_i) and one signature checks prod_i e(PK_i, H(m_i)) e(-G1, sigma) = 1 the same way, without the
-// blinding and the MSM. The DST is fixed: BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_POP_. There is no CPU path.
+// blinding and the MSM. ctt_b200_eth_bls_[batch_]verify_sets check signature sets (fast_aggregate_verify per set) with the public keys
+// gathered by index from a resident registry and summed on the device (sets_verify below, bls_sets_kernels.cuh). The DST is fixed:
+// BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_POP_. There is no CPU path.
 #define CTT_B200_BUILDING_LIBRARY
 #include "../../include/ctt_b200_msm.h"
 #include "msm_hooks.cuh"
 #include "h2c_kernels.cuh"
+#include "bls_sets_kernels.cuh"
 #include "eth_kzg_host.hpp"
 #include "host_pairing.hpp"
+#include <algorithm>
 #include <chrono>
 #include <vector>
 
 namespace b200 {
 B200_DECLARE_CURVE(Bls12381G2)
+void bases_points(const ctt_b200_bases* bases, int* curve_id, size_t* len, const void** d_points);   // msm_capi.cu
 
 namespace ethbls {
 
@@ -113,6 +118,43 @@ static void neg_generator(uint8_t out[PK_BYTES]) {
 
 struct DeviceTimes { float ms_hash = 0, ms_blind = 0, ms_miller = 0, ms_final = 0; };
 
+static void read_times(DeviceTimes* times, cudaEvent_t ev[5]) {
+  cudaEventElapsedTime(&times->ms_hash, ev[0], ev[1]);
+  cudaEventElapsedTime(&times->ms_blind, ev[1], ev[2]);
+  cudaEventElapsedTime(&times->ms_miller, ev[2], ev[3]);
+  cudaEventElapsedTime(&times->ms_final, ev[3], ev[4]);
+}
+
+// Hash n messages to G2 on the device: their expand_message_xmd outputs (host, n x 256 bytes) go through d_uni (device, the same size)
+// into the affine G2 points d_out[0..n-1].
+static void hash_device(cudaStream_t s, const uint8_t* uniform, size_t n, void* d_uni, void* d_out) {
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_uni, uniform, n * UNIFORM_BYTES, cudaMemcpyHostToDevice, s));
+  bls::k_bls_hash_to_g2<<<(unsigned)((n + bls::H2C_THREADS - 1) / bls::H2C_THREADS), bls::H2C_THREADS, 0, s>>>(
+      (const uint8_t*)d_uni, n, (uint32_t*)d_out);
+  B200_CUDA_CHECK(cudaGetLastError());
+}
+
+// The Miller loops of the npairs device pairs (d_g1[i], d_g2[i]) into d_f, ev_miller, then levels of the tree product until `until`
+// values remain: 1 gives the whole product, npairs / 2 the products of pairs 2i and 2i + 1. d_f2 is scratch of (npairs + 1) / 2
+// values. Returns the buffer that holds the result (d_f or d_f2).
+static void* miller_product_device(cudaStream_t s, const void* d_g1, const void* d_g2, size_t npairs, size_t until, void* d_f,
+                                   void* d_f2, cudaEvent_t ev_miller) {
+  bls::k_bls_miller<<<(unsigned)((npairs + bls::PAIR_THREADS - 1) / bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>(
+      (const uint32_t*)d_g1, (const uint32_t*)d_g2, npairs, (uint32_t*)d_f);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(ev_miller, s));
+  size_t m = npairs;
+  while (m > until) {
+    const size_t half = (m + 1) / 2;
+    bls::k_bls_fold<<<(unsigned)((half + bls::PAIR_THREADS - 1) / bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>(
+        (const uint32_t*)d_f, m, (uint32_t*)d_f2);
+    B200_CUDA_CHECK(cudaGetLastError());
+    std::swap(d_f, d_f2);
+    m = half;
+  }
+  return d_f;
+}
+
 // The device part of both verifications, on one engine lease and stream. g1: n + 1 affine G1 points (host) -- with blind, the n
 // public keys are replaced on the device by [r_i]PK_i; uniform: n x 256 bytes hashed to G2 into pairs 0..n-1; g2_last: the affine G2
 // point of pair n. Returns prod e(P_i, Q_i) == 1. gt_out (if not null) receives the GT value e^3 (576 bytes).
@@ -137,10 +179,7 @@ static bool pairing_device(const uint8_t* g1, const uint8_t* uniform, size_t n_h
   B200_CUDA_CHECK(cudaEventRecord(ev[0], s));
   if (n_hashed) {
     B200_CUDA_CHECK(cudaMalloc(&d_uni, n_hashed * UNIFORM_BYTES + 16));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d_uni, uniform, n_hashed * UNIFORM_BYTES, cudaMemcpyHostToDevice, s));
-    bls::k_bls_hash_to_g2<<<(unsigned)((n_hashed + bls::H2C_THREADS - 1) / bls::H2C_THREADS), bls::H2C_THREADS, 0, s>>>(
-        (const uint8_t*)d_uni, n_hashed, (uint32_t*)d_g2);
-    B200_CUDA_CHECK(cudaGetLastError());
+    hash_device(s, uniform, n_hashed, d_uni, d_g2);
   }
   B200_CUDA_CHECK(cudaEventRecord(ev[1], s));
   if (blind) {
@@ -151,32 +190,15 @@ static bool pairing_device(const uint8_t* g1, const uint8_t* uniform, size_t n_h
     B200_CUDA_CHECK(cudaGetLastError());
   }
   B200_CUDA_CHECK(cudaEventRecord(ev[2], s));
-  bls::k_bls_miller<<<(unsigned)((npairs + bls::PAIR_THREADS - 1) / bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>(
-      (const uint32_t*)d_g1, (const uint32_t*)d_g2, npairs, (uint32_t*)d_f);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(ev[3], s));
-  size_t m = npairs;
-  while (m > 1) {
-    const size_t half = (m + 1) / 2;
-    bls::k_bls_fold<<<(unsigned)((half + bls::PAIR_THREADS - 1) / bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>(
-        (const uint32_t*)d_f, m, (uint32_t*)d_f2);
-    B200_CUDA_CHECK(cudaGetLastError());
-    std::swap(d_f, d_f2);
-    m = half;
-  }
-  bls::k_bls_final_exp<<<1, 32, 0, s>>>((const uint32_t*)d_f, (uint32_t*)d_gt, d_flag);
+  const void* d_prod = miller_product_device(s, d_g1, d_g2, npairs, 1, d_f, d_f2, ev[3]);
+  bls::k_bls_final_exp<<<1, 32, 0, s>>>((const uint32_t*)d_prod, (uint32_t*)d_gt, d_flag);
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaEventRecord(ev[4], s));
   int flag = 0;
   B200_CUDA_CHECK(cudaMemcpyAsync(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
   if (gt_out) B200_CUDA_CHECK(cudaMemcpyAsync(gt_out, d_gt, 576, cudaMemcpyDeviceToHost, s));
   B200_CUDA_CHECK(cudaStreamSynchronize(s));
-  if (times) {
-    cudaEventElapsedTime(&times->ms_hash, ev[0], ev[1]);
-    cudaEventElapsedTime(&times->ms_blind, ev[1], ev[2]);
-    cudaEventElapsedTime(&times->ms_miller, ev[2], ev[3]);
-    cudaEventElapsedTime(&times->ms_final, ev[3], ev[4]);
-  }
+  if (times) read_times(times, ev);
   for (auto& e : ev) cudaEventDestroy(e);
   cudaFree(d_g1); cudaFree(d_g2); cudaFree(d_f); cudaFree(d_f2); cudaFree(d_gt); cudaFree(d_flag);
   if (d_uni) cudaFree(d_uni);
@@ -247,6 +269,168 @@ uint8_t aggregate_verify(const uint8_t* pubkeys, const Span* messages, size_t le
   return ok ? Success : VerificationFailure;
 }
 
+// ---- signature sets over a resident registry: fast_aggregate_verify per set ------------------------------------------------------
+// Set i uses the counts[i] registry rows listed in idx after those of sets 0..i-1, messages[i] and signatures[i]. Host: the call-level
+// and per-set input checks, expand_message_xmd, the chunk list of the sets that passed them; in batch mode the blinding chain and
+// sum r_i sigma_i (one G2 MSM). Device, one lease and stream: hash to G2, the key aggregation (bls_sets_kernels.cuh) straight into the
+// G1 slots of the pairs, the Miller loops, then
+//   batch (rnd):     pairs ([r_i]AggPK_i, H(m_i)) and (-G1, sum r_i sigma_i), the whole product, one final exponentiation;
+//   per set (!rnd): pairs 2i = (AggPK_i, H(m_i)) and 2i + 1 = (-G1, sigma_i), one product level, one final exponentiation per set.
+// A set that failed an input check has no chunks, so its G1 slot holds infinity; its status comes from the host.
+static uint8_t sets_verify(const ctt_b200_bases* registry, const uint64_t* idx, const size_t* counts, const Span* messages,
+                           const uint8_t* signatures, size_t n, const uint8_t* rnd, uint8_t* statuses, size_t* failed_set) {
+  if (n == 0) return ZeroLengthAggregation;
+  if (!registry || !idx || !counts || !messages || !signatures || (!rnd && !statuses) || !messages_ok(messages, n))
+    return InputsLengthsMismatch;
+  int curve_id;
+  size_t reg_len;
+  const void* d_reg;
+  bases_points(registry, &curve_id, &reg_len, &d_reg);
+  const size_t LIMIT = 0x7fffffff;
+  if (curve_id != CTT_B200_BLS12_381_G1 || n > LIMIT) return InputsLengthsMismatch;
+  size_t total = 0;
+  for (size_t i = 0; i < n; i++) {
+    if (counts[i] > LIMIT - total) return InputsLengthsMismatch;
+    total += counts[i];
+  }
+
+  Timing t;
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<uint8_t> st(n, Success);
+  std::vector<uint4> chunks;
+  std::vector<uint32_t> chunk_begin(n + 1);
+  for (size_t i = 0, off = 0; i < n; off += counts[i], i++) {
+    chunk_begin[i] = (uint32_t)chunks.size();
+    for (size_t k = 0; k < counts[i]; k++)
+      if (idx[off + k] >= reg_len) { st[i] = InputsLengthsMismatch; break; }
+    if (st[i] == Success && counts[i] == 0) st[i] = ZeroLengthAggregation;
+    if (st[i] == Success && all_zero(signatures + SIG_BYTES * i, SIG_BYTES)) st[i] = PointAtInfinity;
+    if (st[i] != Success) continue;
+    for (size_t k = 0; k < counts[i]; k += bls::SET_CHUNK)
+      chunks.push_back(make_uint4((uint32_t)(off + k), (uint32_t)std::min<size_t>(bls::SET_CHUNK, counts[i] - k), (uint32_t)i, 0));
+  }
+  chunk_begin[n] = (uint32_t)chunks.size();
+  std::vector<uint8_t> uniform;
+  expand_all(uniform, messages, n);
+  std::vector<uint64_t> r;
+  if (rnd) {
+    r.resize(n);
+    blinding_chain(r.data(), n, rnd);
+  }
+  // the host images of the G1 and G2 slots: -G1 and the signatures (or their blinded sum) where the device writes nothing
+  const size_t npairs = rnd ? n + 1 : 2 * n;
+  std::vector<uint8_t> g1(npairs * PK_BYTES, 0), g2;
+  uint8_t neg_g1[PK_BYTES];
+  neg_generator(neg_g1);
+  if (rnd) memcpy(&g1[n * PK_BYTES], neg_g1, PK_BYTES);
+  else for (size_t i = 0; i < n; i++) memcpy(&g1[(2 * i + 1) * PK_BYTES], neg_g1, PK_BYTES);
+  t.ms_host = (float)ms_since(t0);
+  bool sum_inf = false;
+  if (rnd) {
+    const auto t1 = std::chrono::steady_clock::now();
+    std::vector<uint64_t> coefs(4 * n, 0);
+    for (size_t i = 0; i < n; i++) coefs[4 * i] = r[i];
+    host::HXyzz<HFp2> acc;
+    msm_host<Bls12381G2>(&acc, coefs.data(), signatures, n, false, 2);   // raw XYZZ
+    g2.assign(SIG_BYTES, 0);
+    sum_inf = acc.is_inf();                                                // a neutral sum fails the verification
+    if (!sum_inf) {
+      const HFp2 di = (acc.zz * acc.zzz).inv();
+      const HFp2 x = acc.x * (di * acc.zzz), y = acc.y * (di * acc.zz);
+      memcpy(&g2[0], &x, 96);
+      memcpy(&g2[96], &y, 96);
+    }
+    t.ms_msm = (float)ms_since(t1);
+  }
+
+  EngineLease lease = acquire_engine();
+  Engine& E = *lease.e;
+  cudaStream_t s = E.compute();
+  cudaEvent_t ev[5];
+  for (auto& e : ev) B200_CUDA_CHECK(cudaEventCreate(&e));
+  const size_t nch = chunks.size();
+  void *d_g1, *d_g2, *d_h, *d_uni, *d_f, *d_f2, *d_gt, *d_idx, *d_chunks, *d_cb, *d_part, *d_r = nullptr;
+  int* d_flags;   // key_inf[n], neutral[n], then the pairing flags (1 in batch mode, n per set)
+  B200_CUDA_CHECK(cudaMalloc(&d_g1, npairs * PK_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_g2, npairs * SIG_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_h, rnd ? 16 : n * SIG_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_uni, n * UNIFORM_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_f, npairs * 576 + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_f2, ((npairs + 1) / 2) * 576 + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_gt, 576 + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_idx, total * 8 + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_chunks, nch * sizeof(uint4) + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_cb, (n + 1) * 4 + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_part, nch * 4 * 48 + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_flags, 3 * n * sizeof(int) + 16));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_g1, g1.data(), npairs * PK_BYTES, cudaMemcpyHostToDevice, s));
+  if (rnd) {
+    B200_CUDA_CHECK(cudaMemcpyAsync((char*)d_g2 + n * SIG_BYTES, g2.data(), SIG_BYTES, cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMalloc(&d_r, n * 8 + 16));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d_r, r.data(), n * 8, cudaMemcpyHostToDevice, s));
+  } else {
+    B200_CUDA_CHECK(cudaMemcpy2DAsync((char*)d_g2 + SIG_BYTES, 2 * SIG_BYTES, signatures, SIG_BYTES, SIG_BYTES, n, cudaMemcpyHostToDevice, s));
+  }
+  if (total) B200_CUDA_CHECK(cudaMemcpyAsync(d_idx, idx, total * 8, cudaMemcpyHostToDevice, s));
+  if (nch) B200_CUDA_CHECK(cudaMemcpyAsync(d_chunks, chunks.data(), nch * sizeof(uint4), cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_cb, chunk_begin.data(), (n + 1) * 4, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemsetAsync(d_flags, 0, 3 * n * sizeof(int), s));
+  B200_CUDA_CHECK(cudaEventRecord(ev[0], s));
+  if (rnd) hash_device(s, uniform.data(), n, d_uni, d_g2);
+  else {
+    hash_device(s, uniform.data(), n, d_uni, d_h);
+    B200_CUDA_CHECK(cudaMemcpy2DAsync(d_g2, 2 * SIG_BYTES, d_h, SIG_BYTES, SIG_BYTES, n, cudaMemcpyDeviceToDevice, s));
+  }
+  B200_CUDA_CHECK(cudaEventRecord(ev[1], s));
+  if (nch) {
+    bls::k_bls_sets_chunks<<<(unsigned)((nch + bls::SET_CHUNK_THREADS - 1) / bls::SET_CHUNK_THREADS), bls::SET_CHUNK_THREADS, 0, s>>>(
+        (const uint32_t*)d_reg, (const unsigned long long*)d_idx, (const uint4*)d_chunks, nch, (uint32_t*)d_part, d_flags);
+    B200_CUDA_CHECK(cudaGetLastError());
+  }
+  bls::k_bls_sets_finish<<<(unsigned)n, bls::SET_FINISH_THREADS, 0, s>>>((const uint32_t*)d_part, (const uint32_t*)d_cb,
+                                                                         (const unsigned long long*)d_r, (uint32_t*)d_g1,
+                                                                         rnd ? 1 : 2, d_flags + n);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(ev[2], s));
+  const void* d_prod = miller_product_device(s, d_g1, d_g2, npairs, rnd ? 1 : n, d_f, d_f2, ev[3]);
+  if (rnd) bls::k_bls_final_exp<<<1, 32, 0, s>>>((const uint32_t*)d_prod, (uint32_t*)d_gt, d_flags + 2 * n);
+  else bls::k_bls_final_exp_each<<<(unsigned)((n + bls::PAIR_THREADS - 1) / bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>(
+           (const uint32_t*)d_prod, n, d_flags + 2 * n);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(ev[4], s));
+  std::vector<int> flags(3 * n);
+  B200_CUDA_CHECK(cudaMemcpyAsync(flags.data(), d_flags, (rnd ? 2 * n + 1 : 3 * n) * sizeof(int), cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  DeviceTimes dt;
+  read_times(&dt, ev);
+  for (auto& e : ev) cudaEventDestroy(e);
+  for (void* p : {d_g1, d_g2, d_h, d_uni, d_f, d_f2, d_gt, d_idx, d_chunks, d_cb, d_part, (void*)d_flags}) cudaFree(p);
+  if (d_r) cudaFree(d_r);
+  t.ms_hash = dt.ms_hash; t.ms_blind = dt.ms_blind; t.ms_miller = dt.ms_miller; t.ms_final = dt.ms_final;
+  last_timing() = t;
+
+  const int *key_inf = flags.data(), *neutral = flags.data() + n, *ok = flags.data() + 2 * n;
+  for (size_t i = 0; i < n; i++)
+    if (st[i] == Success && key_inf[i]) st[i] = PointAtInfinity;
+  if (rnd) {
+    for (size_t i = 0; i < n; i++)
+      if (st[i] != Success) {
+        if (failed_set) *failed_set = i;
+        return st[i];
+      }
+    for (size_t i = 0; i < n; i++)
+      if (neutral[i]) return VerificationFailure;
+    return ok[0] && !sum_inf ? Success : VerificationFailure;
+  }
+  uint8_t rc = Success;
+  for (size_t i = 0; i < n; i++) {
+    if (st[i] == Success && (neutral[i] || !ok[i])) st[i] = VerificationFailure;
+    statuses[i] = st[i];
+    if (st[i] != Success) rc = VerificationFailure;
+  }
+  return rc;
+}
+
 static int codec_status(int rc) {
   switch (rc) {
     case bls12_381::Success: return CodecSuccess;
@@ -278,6 +462,20 @@ uint8_t ctt_eth_bls_batch_verify_parallel(const void* tp, const void* pubkeys, c
 
 uint8_t ctt_eth_bls_aggregate_verify(const void* pubkeys, const void* messages, size_t len, const void* aggregate_sig) {
   return ethbls::aggregate_verify((const uint8_t*)pubkeys, (const ethbls::Span*)messages, len, (const uint8_t*)aggregate_sig);
+}
+
+uint8_t ctt_b200_eth_bls_batch_verify_sets(const ctt_b200_bases* registry, const uint64_t* key_indices, const size_t* key_counts,
+                                           const void* messages, const void* signatures, size_t n_sets,
+                                           const uint8_t* secure_random_bytes, size_t* failed_set) {
+  if (!secure_random_bytes && n_sets) return ethbls::InputsLengthsMismatch;
+  return ethbls::sets_verify(registry, key_indices, key_counts, (const ethbls::Span*)messages, (const uint8_t*)signatures, n_sets,
+                             secure_random_bytes, nullptr, failed_set);
+}
+
+uint8_t ctt_b200_eth_bls_verify_sets(const ctt_b200_bases* registry, const uint64_t* key_indices, const size_t* key_counts,
+                                     const void* messages, const void* signatures, size_t n_sets, uint8_t* statuses) {
+  return ethbls::sets_verify(registry, key_indices, key_counts, (const ethbls::Span*)messages, (const uint8_t*)signatures, n_sets,
+                             nullptr, statuses, nullptr);
 }
 
 int ctt_b200_eth_bls_deserialize_pubkey_compressed(void* pubkey, const unsigned char src[48]) {

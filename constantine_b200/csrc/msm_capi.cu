@@ -28,6 +28,15 @@ void bases_view(const ctt_b200_bases* bases, const void** d_points, size_t* tabl
   *table_stride = b->d_table ? b->len : 0;
   *force_c = b->d_table ? b->table_c : 0;
 }
+
+// what a gather by index reads (the BLS signature sets, eth_bls.cu): the curve, the number of points and row 0 of the bases, which
+// is the points themselves with or without a window table
+void bases_points(const ctt_b200_bases* bases, int* curve_id, size_t* len, const void** d_points) {
+  const Bases* b = reinterpret_cast<const Bases*>(bases);
+  *curve_id = b->curve_id;
+  *len = b->len;
+  *d_points = b->d_table ? b->d_table : b->d_points;
+}
 }  // namespace b200
 
 #include "msm_capi_generated.inc"

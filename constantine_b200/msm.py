@@ -370,6 +370,59 @@ def eth_bls_aggregate_verify(pubkeys, messages, aggregate_sig: bytes) -> bool:
     return st == 0
 
 
+def _eth_bls_sets(registry, sets):
+    """The C arrays of a list of signature sets (indices, message, signature struct) over a CachedBases registry of BLS12-381 G1
+    public keys. Wrong sizes or a registry of another curve raise ValueError."""
+    if not isinstance(registry, CachedBases) or registry.curve.name != "bls12_381_g1" or not registry._h:
+        raise ValueError("the registry is a CachedBases of bls12_381_g1 public keys")
+    indices, counts, msgs, sigs = [], [], [], []
+    for k, (idx, msg, sig) in enumerate(sets):
+        idx = [int(x) for x in idx]
+        if any(x < 0 or x >= 1 << 64 for x in idx):
+            raise ValueError("set %d: a key index is not a uint64" % k)
+        indices += idx
+        counts.append(len(idx))
+        msgs.append(bytes(msg))
+        sigs.append(sig)
+    if len(counts) > 0x7fffffff or len(indices) > 0x7fffffff:
+        raise ValueError("more than 2^31 - 1 sets or keys")
+    sg = _eth_bls_items(sigs, ETH_BLS_SIGNATURE_BYTES, "signature")
+    spans, keep = _eth_bls_spans(msgs)
+    idx_arr = (ctypes.c_uint64 * max(1, len(indices)))(*indices)
+    cnt_arr = (ctypes.c_size_t * max(1, len(counts)))(*counts)
+    return idx_arr, cnt_arr, spans, ctypes.create_string_buffer(sg or b"\0", max(1, len(sg))), len(counts), keep
+
+
+def eth_bls_batch_verify_sets(registry, sets, secure_random_bytes: bytes) -> bool:
+    """ctt_b200_eth_bls_batch_verify_sets: every set (indices into the registry, message, 192-byte signature struct) is a
+    fast_aggregate_verify, checked together with one blinding scalar per set. registry: CachedBases("bls12_381_g1", pubkey_structs).
+    True on Success, False on VerificationFailure. A set that fails its input checks (status 2 index out of range, 3 no keys, 4 an
+    infinity signature or key) raises ValueError((status, failed_set)) for the lowest such set; no sets raise ValueError((3, None))."""
+    if len(secure_random_bytes) != 32:
+        raise ValueError("secure_random_bytes is 32 bytes, got %d" % len(secure_random_bytes))
+    idx, cnt, spans, sg, n, _keep = _eth_bls_sets(registry, sets)
+    failed = ctypes.c_size_t(ctypes.c_size_t(-1).value)
+    st = _lib.load().ctt_b200_eth_bls_batch_verify_sets(registry._h, idx, cnt, spans, sg, n, _buf(bytes(secure_random_bytes)),
+                                                         ctypes.byref(failed))
+    if st in (0, 1):
+        return st == 0
+    raise ValueError((st, None if failed.value == ctypes.c_size_t(-1).value else failed.value))
+
+
+def eth_bls_verify_sets(registry, sets) -> list:
+    """ctt_b200_eth_bls_verify_sets: the reference's fast_aggregate_verify status of every set (0 Success, 1 VerificationFailure,
+    2 a key index out of range, 3 no keys, 4 an infinity signature or key), no blinding. Arguments as eth_bls_batch_verify_sets;
+    no sets give []."""
+    idx, cnt, spans, sg, n, _keep = _eth_bls_sets(registry, sets)
+    if n == 0:
+        return []
+    out = ctypes.create_string_buffer(n)
+    st = _lib.load().ctt_b200_eth_bls_verify_sets(registry._h, idx, cnt, spans, sg, n, out)
+    if st not in (0, 1):
+        raise ValueError(st)
+    return list(out.raw)
+
+
 def eth_bls_last_timing() -> dict:
     """Host checks with expand_message_xmd and the blinding chain, device hash to G2, blinding, Miller loops, final exponentiation
     (CUDA events) and the G2 MSM (ms) of the calling thread's last BLS verification."""
