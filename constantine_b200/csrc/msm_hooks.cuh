@@ -147,6 +147,7 @@ __global__ void __launch_bounds__(128) k_scalar_mul_u64(const uint32_t* base, co
 template <class C>
 int run_scalar_mul_u64(const void* base_aff, const void* k, size_t count, void* out_aff) {
   using T = typename C::T;
+  if (count == 0) return 0;   // nothing to compute (an empty grid is not a valid launch)
   EngineLease lease = acquire_engine();
   Engine& E = *lease.e;
   size_t pt = 2 * C::COORD_BYTES;
