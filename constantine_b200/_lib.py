@@ -159,6 +159,12 @@ def load():
     lib.ctt_b200_eth_bls_batch_verify_sets.restype = ub
     lib.ctt_b200_eth_bls_verify_sets.argtypes = [vp, vp, vp, vp, vp, sz, vp]
     lib.ctt_b200_eth_bls_verify_sets.restype = ub
+    lib.ctt_b200_eth_bls_deserialize_pubkeys_compressed_batch.argtypes = [vp, vp, vp, sz]
+    lib.ctt_b200_eth_bls_deserialize_pubkeys_compressed_batch.restype = ci
+    lib.ctt_b200_eth_bls_deserialize_signatures_compressed_batch.argtypes = [vp, vp, vp, sz]
+    lib.ctt_b200_eth_bls_deserialize_signatures_compressed_batch.restype = ci
+    lib.ctt_b200_eth_bls_registry_from_compressed.argtypes = [vp, sz, vp, ctypes.POINTER(sz), ctypes.POINTER(ci)]
+    lib.ctt_b200_eth_bls_registry_from_compressed.restype = vp
     lib.ctt_b200_test_hash_to_g2.argtypes = [vp, sz, vp, sz, vp]
     lib.ctt_b200_test_hash_to_g2.restype = ci
     lib.ctt_b200_test_map_to_g2.argtypes = [vp, sz, vp]

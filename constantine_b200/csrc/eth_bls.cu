@@ -11,13 +11,16 @@
 //           loops, their tree product and the final exponentiation (pairing_kernels.cuh); one flag comes back.
 // aggregate_verify of n pairs (PK_i, m_i) and one signature checks prod_i e(PK_i, H(m_i)) e(-G1, sigma) = 1 the same way, without the
 // blinding and the MSM. ctt_b200_eth_bls_[batch_]verify_sets check signature sets (fast_aggregate_verify per set) with the public keys
-// gathered by index from a resident registry and summed on the device (sets_verify below, bls_sets_kernels.cuh). The DST is fixed:
+// gathered by index from a resident registry and summed on the device (sets_verify below, bls_sets_kernels.cuh).
+// ctt_b200_eth_bls_deserialize_{pubkeys,signatures}_compressed_batch and ctt_b200_eth_bls_registry_from_compressed decode compressed
+// points on the device, one thread per point (codec_kernels.cuh); the registry's keys go straight into a ctt_b200_bases handle. The DST is fixed:
 // BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_POP_. There is no CPU path.
 #define CTT_B200_BUILDING_LIBRARY
 #include "../../include/ctt_b200_msm.h"
 #include "msm_hooks.cuh"
 #include "h2c_kernels.cuh"
 #include "bls_sets_kernels.cuh"
+#include "codec_kernels.cuh"
 #include "eth_kzg_host.hpp"
 #include "host_pairing.hpp"
 #include <algorithm>
@@ -27,6 +30,7 @@
 namespace b200 {
 B200_DECLARE_CURVE(Bls12381G2)
 void bases_points(const ctt_b200_bases* bases, int* curve_id, size_t* len, const void** d_points);   // msm_capi.cu
+ctt_b200_bases* bases_wrap(int curve_id, size_t len, void* d_points);                                // msm_capi.cu
 
 namespace ethbls {
 
@@ -441,6 +445,75 @@ static int codec_status(int rc) {
   }
 }
 
+// ---- compressed public keys and signatures decoded on the device (codec_kernels.cuh) ---------------------------------------------
+constexpr size_t PK_COMPRESSED = 48, SIG_COMPRESSED = 96, DECODE_LIMIT = size_t(1) << 31;
+
+// n compressed points (48 bytes each for G1, 96 for G2) -> d_out (n affine structs on the device) and statuses (host), on stream s;
+// returns with everything copied back
+static void decode_device(cudaStream_t s, bool g2, const uint8_t* src, size_t n, void* d_out, uint8_t* statuses) {
+  const size_t in_bytes = g2 ? SIG_COMPRESSED : PK_COMPRESSED;
+  void *d_src, *d_st;
+  B200_CUDA_CHECK(cudaMalloc(&d_src, n * in_bytes + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_st, n + 16));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_src, src, n * in_bytes, cudaMemcpyHostToDevice, s));
+  const unsigned blocks = (unsigned)((n + codec::DECODE_THREADS - 1) / codec::DECODE_THREADS);
+  if (g2) codec::k_bls_decode_g2<<<blocks, codec::DECODE_THREADS, 0, s>>>((const uint8_t*)d_src, n, (uint32_t*)d_out, (uint8_t*)d_st);
+  else codec::k_bls_decode_g1<<<blocks, codec::DECODE_THREADS, 0, s>>>((const uint8_t*)d_src, n, (uint32_t*)d_out, (uint8_t*)d_st);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpyAsync(statuses, d_st, n, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  cudaFree(d_src);
+  cudaFree(d_st);
+}
+
+// the two batch entries: one lease and stream, the structs and statuses back to the host
+static int decode_batch(bool g2, void* out, uint8_t* statuses, const uint8_t* src, size_t n) {
+  if (n == 0) return 0;
+  if (!out || !statuses || !src || n >= DECODE_LIMIT) return -1;
+  const size_t out_bytes = g2 ? SIG_BYTES : PK_BYTES;
+  EngineLease lease = acquire_engine();
+  Engine& E = *lease.e;
+  cudaStream_t s = E.compute();
+  void* d_out;
+  B200_CUDA_CHECK(cudaMalloc(&d_out, n * out_bytes + 16));
+  decode_device(s, g2, src, n, d_out, statuses);
+  B200_CUDA_CHECK(cudaMemcpyAsync(out, d_out, n * out_bytes, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  cudaFree(d_out);
+  for (size_t i = 0; i < n; i++)
+    if (statuses[i] != CodecSuccess) return 1;
+  return 0;
+}
+
+// the registry: the keys are decoded straight into the point buffer of a new handle, which is kept only when every status is 0
+static ctt_b200_bases* registry_from_compressed(const uint8_t* pubkeys, size_t n, uint8_t* statuses, size_t* failed_index, int* status) {
+  if (n == 0 || !pubkeys || n >= DECODE_LIMIT) {
+    if (status) *status = -1;
+    return nullptr;
+  }
+  std::vector<uint8_t> own;
+  if (!statuses) {
+    own.resize(n);
+    statuses = own.data();
+  }
+  void* d_points;
+  {
+    EngineLease lease = acquire_engine();
+    Engine& E = *lease.e;
+    B200_CUDA_CHECK(cudaMalloc(&d_points, n * PK_BYTES + 16));   // the layout of ctt_b200_bases_upload
+    decode_device(E.compute(), false, pubkeys, n, d_points, statuses);
+  }
+  for (size_t i = 0; i < n; i++)
+    if (statuses[i] != CodecSuccess) {   // infinity (5) included: KeyValidate rejects it
+      cudaFree(d_points);
+      if (failed_index) *failed_index = i;
+      if (status) *status = statuses[i];
+      return nullptr;
+    }
+  if (status) *status = CodecSuccess;
+  return bases_wrap(CTT_B200_BLS12_381_G1, n, d_points);
+}
+
 }  // namespace ethbls
 }  // namespace b200
 
@@ -495,6 +568,19 @@ int ctt_b200_eth_bls_deserialize_signature_compressed(void* sig, const unsigned 
   memcpy(sig, &q.x, 96);
   memcpy((char*)sig + 96, &q.y, 96);
   return q.inf() ? ethbls::CodecPointAtInfinity : ethbls::CodecSuccess;
+}
+
+int ctt_b200_eth_bls_deserialize_pubkeys_compressed_batch(void* pubkeys, uint8_t* statuses, const unsigned char* src, size_t n) {
+  return ethbls::decode_batch(false, pubkeys, statuses, src, n);
+}
+
+int ctt_b200_eth_bls_deserialize_signatures_compressed_batch(void* sigs, uint8_t* statuses, const unsigned char* src, size_t n) {
+  return ethbls::decode_batch(true, sigs, statuses, src, n);
+}
+
+ctt_b200_bases* ctt_b200_eth_bls_registry_from_compressed(const unsigned char* pubkeys, size_t n, uint8_t* statuses,
+                                                          size_t* failed_index, int* status) {
+  return ethbls::registry_from_compressed(pubkeys, n, statuses, failed_index, status);
 }
 
 void ctt_b200_eth_bls_last_timing(float* ms_host, float* ms_hash, float* ms_blind, float* ms_msm, float* ms_miller, float* ms_final) {

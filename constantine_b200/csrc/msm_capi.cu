@@ -37,6 +37,16 @@ void bases_points(const ctt_b200_bases* bases, int* curve_id, size_t* len, const
   *len = b->len;
   *d_points = b->d_table ? b->d_table : b->d_points;
 }
+
+// a handle around len points already on the device (the registry decoded from compressed keys, eth_bls.cu): d_points is a cudaMalloc
+// buffer of the layout ctt_b200_bases_upload makes, and ctt_b200_bases_free releases it
+ctt_b200_bases* bases_wrap(int curve_id, size_t len, void* d_points) {
+  Bases* b = new Bases;
+  b->curve_id = curve_id;
+  b->len = len;
+  b->d_points = d_points;
+  return reinterpret_cast<ctt_b200_bases*>(b);
+}
 }  // namespace b200
 
 #include "msm_capi_generated.inc"

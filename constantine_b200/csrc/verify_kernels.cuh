@@ -3,9 +3,9 @@
 //   e(sum_k r^k pi_k, [tau^64]G2) = e(sum_k r^k h_k^64 pi_k + sum_i (sum_{k in row i} r^k) C_i - [sum_k r^k I_k(tau)]G1, G2).
 // Per call, on one engine lease and stream:
 //   1. k_ver_decode: one thread per point (the n proofs, then the U unique commitments): the host has done the byte-level part of the
-//      compressed format (flags, x < p); the kernel takes y = (x^3 + 4)^((p+1)/4), checks it, picks the sign and checks [r]P = O with
-//      the XYZZ formulas (the same double-and-add chain as the host's in_subgroup), and writes the affine point straight into the
-//      MSM point set, plus one status byte per point. The cells are parsed (k_kzg_parse) behind it while the host hashes.
+//      compressed format (flags, x < p); the kernel runs the shared G1 decoder of codec_g1.cuh (y = (x^3 + 4)^((p+1)/4), checked,
+//      the sign, and the endomorphism subgroup test, which accepts exactly the points the host's [r]P = O accepts), and writes the
+//      affine point straight into the MSM point set, plus one status byte per point. The cells are parsed (k_kzg_parse) behind it while the host hashes.
 //   2. after the host has read the statuses and chosen r: k_ver_powers (r^1 .. r^n), k_ver_scalars (row A = r^k; row B = r^k h_k^64 and
 //      the per-commitment sums of r^k), k_ver_columns (one block per used column: sum_k r^k evals_k, the 64-point coset inverse NTT with
 //      shift h_c = w8192^brp7(c)), k_ver_interp (the column results summed and negated into row B);
@@ -16,6 +16,7 @@
 // Included by inst_bls12_381_g1.cu only, next to the engine instantiation it runs.
 #pragma once
 #include "peerdas_kernels.cuh"
+#include "codec_g1.cuh"
 
 namespace b200 {
 namespace kzg {
@@ -23,65 +24,23 @@ namespace kzg {
 using FpD = Fp<Bls12381Fp>;
 constexpr int VER_THREADS = 128;
 
-// p's words with a small constant added and shifted right: ((p + add) >> shift), 12 little-endian 32-bit words
-__device__ __forceinline__ void ver_p_words(uint32_t* e, uint32_t add, int shift) {
-  uint64_t carry = add;
-#pragma unroll
-  for (int i = 0; i < 12; i++) { const uint64_t v = (uint64_t)Bls12381Fp::P(i) + carry; e[i] = (uint32_t)v; carry = v >> 32; }
-#pragma unroll
-  for (int i = 0; i < 12; i++) e[i] = (e[i] >> shift) | (i + 1 < 12 ? e[i + 1] << (32 - shift) : 0u);
-}
-
-// in: per point VER_IN_WORDS words (kzg_device.hpp, VerifyPoint); pts: affine Montgomery (x, y), (0, 0) for infinity; status: per point
+// in: per point VER_IN_WORDS words (kzg_device.hpp, VerifyPoint); pts: affine Montgomery (x, y), (0, 0) for infinity; status: per point,
+// the cttEthKzg statuses (codec_g1.cuh's not on the curve -> 7, not in the subgroup -> 8)
 __global__ void __launch_bounds__(VER_THREADS) k_ver_decode(const VerifyPoint* __restrict__ in, size_t count, uint32_t* pts, uint8_t* status) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
   const VerifyPoint v = in[i];
   uint32_t* o = pts + i * 2 * FpD::WORDS;
-  if (v.mode != VER_DECODE) {                         // infinity (valid) or a status the host has already found
-    store_words(o, FpD::zero());
-    store_words(o + FpD::WORDS, FpD::zero());
-    status[i] = v.mode == VER_INFINITY ? (uint8_t)0 : (uint8_t)v.mode;
-    return;
+  FpD x = FpD::zero(), y = FpD::zero();
+  uint8_t st;
+  if (v.mode != VER_DECODE) st = v.mode == VER_INFINITY ? (uint8_t)0 : (uint8_t)v.mode;   // infinity, or a status the host found
+  else {
+    const int rc = codec::g1_decode(v.x, v.sign != 0, x, y);
+    st = rc == codec::CODEC_OK ? 0 : (rc == codec::CODEC_NOT_ON_CURVE ? 7 : 8);
   }
-  FpD x, r2, one_raw = FpD::zero();
-#pragma unroll
-  for (int w = 0; w < 12; w++) { x.l[w] = v.x[w]; r2.l[w] = Bls12381Fp::R2(w); }
-  one_raw.l[0] = 1;
-  x = x.mul_u(r2);
-  FpD four = FpD::one().dbl();
-  four = four.dbl();
-  const FpD rhs = x.sqr() * x + four;
-  uint32_t e[12];
-  ver_p_words(e, 1, 2);                               // (p + 1) / 4
-  FpD y = FpD::one();
-#pragma unroll 1
-  for (int b = 380; b >= 0; b--) {
-    y = y.sqr();
-    if ((e[b >> 5] >> (b & 31)) & 1u) y = y * rhs;
-  }
-  if (!(y.sqr() == rhs)) { status[i] = 7; store_words(o, FpD::zero()); store_words(o + FpD::WORDS, FpD::zero()); return; }
-  // sign: y > (p - 1) / 2 as integers
-  const FpD yc = y.mul_u(one_raw);
-  ver_p_words(e, 0, 1);                               // (p - 1) / 2 (p is odd: the shift drops the 1)
-  bool larger = false;
-#pragma unroll 1
-  for (int w = 11; w >= 0; w--) {
-    if (yc.l[w] != e[w]) { larger = yc.l[w] > e[w]; break; }
-  }
-  if (larger != (v.sign != 0)) y = y.neg();
-  // [r]P = O, r = the group order, by double-and-add from the top bit (host_bls12_381.hpp in_subgroup)
-  Xyzz<FpD> base, acc = Xyzz<FpD>::inf();
-  base.x = x; base.y = y; base.zz = FpD::one(); base.zzz = FpD::one();
-#pragma unroll 1
-  for (int b = 254; b >= 0; b--) {
-    acc = xyzz_dbl_u(acc);
-    if ((Bls12381Fr::P(b >> 5) >> (b & 31)) & 1u) xyzz_add_u(acc, base);
-  }
-  const bool ok = acc.is_inf();
-  store_words(o, ok ? x : FpD::zero());
-  store_words(o + FpD::WORDS, ok ? y : FpD::zero());
-  status[i] = ok ? 0 : 8;
+  store_words(o, x);
+  store_words(o + FpD::WORDS, y);
+  status[i] = st;
 }
 
 // rp[k] = r^(k + 1) for k < n (the reference's powers skip r^0): square-and-multiply on k + 1 per thread

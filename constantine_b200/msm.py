@@ -162,6 +162,13 @@ class CachedBases:
         self.n = length if length is not None else len(memoryview(points).cast("B")) // self.curve.aff_bytes
         self._h = _lib.load().ctt_b200_bases_upload(self.curve.curve_id, _buf(points), self.n)
 
+    @classmethod
+    def _from_handle(cls, curve, handle, n):
+        """Wrap a ctt_b200_bases handle that a C entry made (eth_bls_registry_from_compressed); free() releases it."""
+        self = cls.__new__(cls)
+        self.curve, self.n, self._h = _curve(curve), n, handle
+        return self
+
     def precompute(self, c: int = 0, msm_len: int = 0) -> int:
         """One-time table of window multiples 2^(c w) P_i (ctt_b200_bases_precompute[_for]); returns the window size
         used. msm_len: length of the MSMs the bases will serve when they hold a whole bank (default: all bases)."""
@@ -321,6 +328,61 @@ def eth_bls_deserialize_signature(b96: bytes) -> bytes:
     if st != 0:
         raise ValueError(st)
     return out.raw
+
+
+def _compressed_items(items, size, what):
+    """A list of compressed points, or one joined buffer of them, as (bytes, count); a wrong size raises ValueError."""
+    if isinstance(items, (bytes, bytearray, memoryview)):
+        b = bytes(items)
+        if len(b) % size:
+            raise ValueError("joined compressed %ss: %d bytes is not a multiple of %d" % (what, len(b), size))
+        return b, len(b) // size
+    items = [bytes(x) for x in items]
+    for x in items:
+        if len(x) != size:
+            raise ValueError("a compressed %s is %d bytes, got %d" % (what, size, len(x)))
+    return b"".join(items), len(items)
+
+
+def _deserialize_batch(fn, items, in_size, out_size, what):
+    src, n = _compressed_items(items, in_size, what)
+    if n == 0:
+        return [], []
+    out = ctypes.create_string_buffer(out_size * n)
+    st = ctypes.create_string_buffer(n)
+    rc = fn(out, st, _buf(src), n)
+    if rc not in (0, 1):
+        raise ValueError("%s batch: %d items rejected by the C entry (rc %d)" % (what, n, rc))
+    raw = out.raw
+    return [raw[out_size * i:out_size * (i + 1)] for i in range(n)], list(st.raw)
+
+
+def eth_bls_deserialize_pubkeys(b48s):
+    """Compressed public keys decoded on the GPU (ctt_b200_eth_bls_deserialize_pubkeys_compressed_batch): b48s is a list of 48-byte
+    keys or one joined buffer of them. Returns (structs, statuses): the 96-byte ctt_eth_bls_pubkey of every key (all zeros unless its
+    status is 0) and its ctt_codec_ecc_status, as eth_bls_deserialize_pubkey reports it."""
+    return _deserialize_batch(_lib.load().ctt_b200_eth_bls_deserialize_pubkeys_compressed_batch, b48s, 48, ETH_BLS_PUBKEY_BYTES,
+                              "public key")
+
+
+def eth_bls_deserialize_signatures(b96s):
+    """Compressed signatures decoded on the GPU (ctt_b200_eth_bls_deserialize_signatures_compressed_batch), as
+    eth_bls_deserialize_pubkeys: (192-byte ctt_eth_bls_signature structs, statuses)."""
+    return _deserialize_batch(_lib.load().ctt_b200_eth_bls_deserialize_signatures_compressed_batch, b96s, 96, ETH_BLS_SIGNATURE_BYTES,
+                              "signature")
+
+
+def eth_bls_registry_from_compressed(pubkeys) -> "CachedBases":
+    """A signature-set registry decoded on the GPU from compressed public keys (ctt_b200_eth_bls_registry_from_compressed): a
+    CachedBases of bls12_381_g1 holding the rows CachedBases("bls12_381_g1", structs) would hold. The keys never return to the host.
+    A key whose status is not 0 (infinity, 5, included) raises ValueError((status, index)) for the lowest such key; no keys raise
+    ValueError((-1, None))."""
+    src, n = _compressed_items(pubkeys, 48, "public key")
+    failed, status = ctypes.c_size_t(0), ctypes.c_int(0)
+    h = _lib.load().ctt_b200_eth_bls_registry_from_compressed(_buf(src or b"\0"), n, None, ctypes.byref(failed), ctypes.byref(status))
+    if not h:
+        raise ValueError((status.value, None if status.value < 0 else failed.value))
+    return CachedBases._from_handle("bls12_381_g1", h, n)
 
 
 def _eth_bls_items(items, size, what):

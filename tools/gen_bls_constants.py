@@ -10,6 +10,9 @@ Nothing here is copied from a table: every constant is computed from the curve.
   - psi(x, y) = (conj(x) cx, conj(y) cy) with cx = (1 + i)^(-(p - 1) / 3), cy = (1 + i)^(-(p - 1) / 2) (the untwist-Frobenius-twist
     endomorphism of the cofactor clearing, Budroni-Pintore).
   - The Frobenius of Fp12 = Fp2[w] / (w^6 - (1 + i)): w^k -> gamma_k w^k with gamma_k = (1 + i)^(k (p - 1) / 6), k = 1..5.
+  - beta, the cube root of unity of Fp for which phi(x, y) = (beta x, y) acts on G1 as [-u^2] (u = -X_ABS): the G1 subgroup test of
+    Scott (eprint 2021/1130) checks phi(P) = [-u^2]P. Of the two primitive cube roots exactly one does; the generator asserts it on
+    the G1 generator. It goes to constantine_b200/csrc/codec_constants.cuh (the decoders of codec_g1.cuh / codec_kernels.cuh).
 """
 import json
 import os
@@ -22,6 +25,9 @@ R = 0x73eda753299d7d483339d80809a1d80553bda402fffe5bfeffffffff00000001
 X_ABS = 0xd201000000010000                     # the curve parameter is x = -X_ABS
 FIXTURE = os.path.join(ROOT, "tests", "golden", "bls_kat.json")
 OUT = os.path.join(ROOT, "constantine_b200", "csrc", "bls_constants.cuh")
+OUT_CODEC = os.path.join(ROOT, "constantine_b200", "csrc", "codec_constants.cuh")
+G1_GEN = (0x17f1d3a73197d7942695638c4fa9ac0fc3688c4f9774b905a14e3a3f171bac586c55e83ff97a1aeffb3af00adb22c6bb,
+          0x08b3f481e3aaa0f1a09e30ed741d8ae4fcf5e095d5d00af600db18cb2c04b3edd03cc744a2888ae40caa232946c5e7e1)
 
 
 # ---- Fp2 = Fp[i] / (i^2 + 1) as pairs --------------------------------------------------------------------------------------
@@ -301,6 +307,48 @@ def frobenius_constants():
     return [fpow(XI, k * (P - 1) // 6) for k in range(1, 6)]
 
 
+# ---- G1 (y^2 = x^3 + 4 over Fp), affine, None is infinity: only what the choice of beta needs -----------------------------------
+def g1_add(p1, p2):
+    if p1 is None:
+        return p2
+    if p2 is None:
+        return p1
+    (x1, y1), (x2, y2) = p1, p2
+    if x1 == x2:
+        if (y1 + y2) % P == 0:
+            return None
+        lam = 3 * x1 * x1 * pow(2 * y1, -1, P) % P
+    else:
+        lam = (y2 - y1) * pow(x2 - x1, -1, P) % P
+    x3 = (lam * lam - x1 - x2) % P
+    return x3, (lam * (x1 - x3) - y1) % P
+
+
+def g1_mul(k, pt):
+    if k < 0:
+        k, pt = -k, (None if pt is None else (pt[0], (-pt[1]) % P))
+    acc = None
+    for bit in bin(k)[2:] if k else "":
+        acc = g1_add(acc, acc)
+        if bit == "1":
+            acc = g1_add(acc, pt)
+    return acc
+
+
+def g1_beta():
+    """The primitive cube root of unity beta with (beta x, y) = [-u^2](x, y) on G1, asserted on the generator."""
+    g = 2
+    while pow(g, (P - 1) // 3, P) == 1:
+        g += 1
+    w = pow(g, (P - 1) // 3, P)
+    target = g1_mul(-(X_ABS * X_ABS), G1_GEN)
+    good = [b for b in (w, w * w % P) if (b * G1_GEN[0] % P, G1_GEN[1]) == target]
+    assert len(good) == 1, "expected exactly one cube root of unity with phi = [-u^2] on G1, found %d" % len(good)
+    beta = good[0]
+    assert beta != 1 and pow(beta, 3, P) == 1
+    return beta
+
+
 def load_rfc_vectors():
     with open(FIXTURE) as f:
         return json.load(f)["rfc_h2c"]["vectors"]
@@ -352,12 +400,35 @@ def header_text():
     return "\n".join(body)
 
 
-def main():
-    text = header_text()
-    old = open(OUT).read() if os.path.exists(OUT) else None
+def codec_header_text():
+    words = mont_words(g1_beta())
+    body = [
+        "// GENERATED by tools/gen_bls_constants.py -- derived from the curve, see that file.",
+        "#pragma once",
+        "#include <cstdint>",
+        "",
+        "namespace b200 {",
+        "namespace codec {",
+        "// beta: the primitive cube root of unity of Fp for which phi(x, y) = (beta x, y) acts on G1 as [-u^2], u = -0xd201000000010000",
+        "// (checked on the generator); Montgomery form (R = 2^384), 12 little-endian 32-bit words",
+        "__device__ __forceinline__ void g1_beta_words(uint32_t w[12]) {",
+    ]
+    for k in range(0, 12, 4):
+        body.append("  " + " ".join("w[%d] = 0x%08xu;" % (k + j, words[k + j]) for j in range(4)))
+    body += ["}", "}  // namespace codec", "}  // namespace b200", ""]
+    return "\n".join(body)
+
+
+def write_if_changed(path, text):
+    old = open(path).read() if os.path.exists(path) else None
     if old != text:
-        with open(OUT, "w") as f:
+        with open(path, "w") as f:
             f.write(text)
+
+
+def main():
+    write_if_changed(OUT, header_text())
+    write_if_changed(OUT_CODEC, codec_header_text())
     print("bls constants: one isogeny of %d candidates matches the RFC vectors" % len(iso_candidates()))
 
 
