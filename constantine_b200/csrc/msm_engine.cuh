@@ -164,6 +164,11 @@ struct Engine {
   cudaStream_t user_stream = nullptr;  // caller-provided compute stream for this lease (ctt_b200_set_stream), or null
   cudaStream_t order_after = nullptr;  // caller's stream this lease only orders itself behind (slots other than slot 0)
   cudaEvent_t ev_order = nullptr;
+  // A lease that returns with its work still queued (a device destination: msm_device sets `unsynced`) records ev_done on its
+  // compute stream when it ends; the caller's stream waits on it (order_after), and so do the streams of the slot's next lease
+  // (`pending`) before their first operation -- which may be on another stream after ctt_b200_set_stream.
+  cudaEvent_t ev_done = nullptr;
+  bool unsynced = false, pending = false;
   cudaStream_t compute() const { return user_stream ? user_stream : stream; }
   cudaEvent_t msm_ev[MSM_MARKS];
   // timing events of the engine's callers (the h2d window of msm_host_on, the phases of the KZG / PeerDAS / verification drivers),
@@ -218,6 +223,7 @@ struct Engine {
     for (auto& x : caller_ev) B200_CUDA_CHECK(cudaEventCreate(&x));
     B200_CUDA_CHECK(cudaEventCreateWithFlags(&ev_points_ready, cudaEventDisableTiming));
     B200_CUDA_CHECK(cudaEventCreateWithFlags(&ev_order, cudaEventDisableTiming));
+    B200_CUDA_CHECK(cudaEventCreateWithFlags(&ev_done, cudaEventDisableTiming));
     for (auto& x : ev_chunk) B200_CUDA_CHECK(cudaEventCreateWithFlags(&x, cudaEventDisableTiming));
     h_result_cap = 1 << 20;
     B200_CUDA_CHECK(cudaMallocHost(&h_result, h_result_cap));
@@ -307,6 +313,19 @@ struct EngineLease {
   std::unique_ptr<DeviceGuard> guard;    // declared first: the device is restored after the slot is released
   Engine* e = nullptr;
   std::unique_lock<std::mutex> lock;
+  EngineLease() = default;
+  EngineLease(EngineLease&& o) noexcept : guard(std::move(o.guard)), e(o.e), lock(std::move(o.lock)) { o.e = nullptr; }
+  EngineLease& operator=(EngineLease&&) = delete;
+  // Work left queued by this lease (a device destination): the caller's stream and the slot's next lease order themselves
+  // behind it. Runs while the slot is still held, before the device is restored.
+  ~EngineLease() {
+    if (!e || !e->unsynced) return;
+    Engine& E = *e;
+    B200_CUDA_CHECK(cudaEventRecord(E.ev_done, E.compute()));
+    if (E.order_after) B200_CUDA_CHECK(cudaStreamWaitEvent(E.order_after, E.ev_done, 0));
+    E.unsynced = false;
+    E.pending = true;
+  }
 };
 
 // Lease a slot of `device` (< 0: the primary device), make that device current, initialise the slot on first use and give it
@@ -338,11 +357,19 @@ inline EngineLease acquire_engine(int device = -1) {
     E.tuning = cfg.tuning;
     // the caller's stream: slot 0 of the primary device launches on it directly; any other slot keeps its own stream but
     // orders itself behind the work already queued on the caller's stream (device-resident inputs may still be in flight)
+    // (the caller's stream belongs to the primary device: the slots of other devices are not ordered against it)
     const bool direct = (slot == 0 && device == cfg.primary_device);
     E.user_stream = direct ? cfg.user_stream : nullptr;
-    E.order_after = direct ? nullptr : cfg.user_stream;
+    E.order_after = (direct || device != cfg.primary_device) ? nullptr : cfg.user_stream;
   }
-  if (E.order_after && device == primary_device()) {
+  if (E.pending) {
+    // the last lease of this slot returned with work queued that reads and writes the slot's scratch; this lease may launch on
+    // another stream (ctt_b200_set_stream since), and its copy stream is never ordered behind the compute stream
+    B200_CUDA_CHECK(cudaStreamWaitEvent(E.compute(), E.ev_done, 0));
+    B200_CUDA_CHECK(cudaStreamWaitEvent(E.copy_stream, E.ev_done, 0));
+    E.pending = false;
+  }
+  if (E.order_after) {
     B200_CUDA_CHECK(cudaEventRecord(E.ev_order, E.order_after));
     B200_CUDA_CHECK(cudaStreamWaitEvent(E.stream, E.ev_order, 0));
   }
@@ -919,6 +946,7 @@ host::HXyzz<typename C::H> msm_device(Engine& E, const MsmJob& job) {
     // the caller's collective (same stream) gathers every rank's digits and ONE host pass combines them
     B200_CUDA_CHECK(cudaMemcpyAsync(job.out, red.parts, (size_t)z.nw * red.per_set * XYZZ_BYTES, cudaMemcpyDeviceToDevice, s));
     st.ms_total = 0;
+    E.unsynced = true;
   } else if (job.batch > 1) {
     // batch: the partial sums + Horner per MSM on the device (one thread per MSM), into the caller's device array or, for the host,
     // into the other reduce buffer (free by now, >= nw points)
@@ -929,6 +957,7 @@ host::HXyzz<typename C::H> msm_device(Engine& E, const MsmJob& job) {
     launches++;
     if (on_device) {
       if (E.collect_timing) B200_CUDA_CHECK(cudaEventRecord(E.msm_ev[MSM_DONE], s));
+      E.unsynced = true;
     } else {
       E.ensure_host(job.batch * XYZZ_BYTES);
       B200_CUDA_CHECK(cudaMemcpyAsync(E.h_result, dst, job.batch * XYZZ_BYTES, cudaMemcpyDeviceToHost, s));

@@ -114,7 +114,8 @@ def digits_per_window(c: int) -> int:
 
 def msm_device_digits(curve, d_digits_out: int, d_coefs: int, d_points: int, n: int, fr_mont=False, force_c=0, win_begin=0, win_end=-1) -> int:
     """Window range [win_begin, win_end) of an MSM over device-resident inputs; the radix-16 digits of the window sums stay in the
-    device buffer d_digits_out (raw XYZZ, window-major). NOT synchronised: order later work on the engine's stream."""
+    device buffer d_digits_out (raw XYZZ, window-major). NOT synchronised: work queued afterwards on the caller's stream
+    (ctt_b200_set_stream) sees the digits; without a caller's stream, synchronise the device before reading them."""
     cv = _curve(curve)
     g = _lib.load().ctt_b200_msm_device_digits(cv.curve_id, d_digits_out, d_coefs, d_points, n, int(fr_mont), force_c, win_begin, win_end)
     if g < 0:
