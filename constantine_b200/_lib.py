@@ -165,6 +165,16 @@ def load():
     lib.ctt_b200_eth_bls_deserialize_signatures_compressed_batch.restype = ci
     lib.ctt_b200_eth_bls_registry_from_compressed.argtypes = [vp, sz, vp, ctypes.POINTER(sz), ctypes.POINTER(ci)]
     lib.ctt_b200_eth_bls_registry_from_compressed.restype = vp
+    lib.ctt_b200_fft_domain_new.argtypes = [ci, vp, ci, ctypes.POINTER(ci)]
+    lib.ctt_b200_fft_domain_new.restype = vp
+    lib.ctt_b200_fft_domain_free.argtypes = [vp]
+    lib.ctt_b200_fft_domain_free.restype = None
+    lib.ctt_b200_fft.argtypes = [vp, ci, vp, vp, sz, sz, vp]
+    lib.ctt_b200_fft.restype = ci
+    lib.ctt_b200_fft_device.argtypes = [vp, ci, vp, vp, sz, sz, vp]
+    lib.ctt_b200_fft_device.restype = ci
+    lib.ctt_b200_fft_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 3
+    lib.ctt_b200_fft_last_timing.restype = None
     lib.ctt_b200_test_hash_to_g2.argtypes = [vp, sz, vp, sz, vp]
     lib.ctt_b200_test_hash_to_g2.restype = ci
     lib.ctt_b200_test_map_to_g2.argtypes = [vp, sz, vp]

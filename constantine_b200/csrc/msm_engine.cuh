@@ -190,6 +190,9 @@ struct Engine {
   DeviceBuffer das_rec, das_z;
   // EIP-7594 batch verification: the inputs (points, cells, index lists, r), the MSM point set, statuses / powers / column results
   DeviceBuffer ver_in, ver_pts, ver_aux;
+  // scalar-field FFTs (fft.cu): the host entry's device copy of the data, the intermediate of the nn kinds above 4096 points and a
+  // call's coset factors
+  DeviceBuffer fft_data, fft_scratch, fft_tab;
   void* h_result = nullptr;   // pinned
   size_t h_result_cap = 0;
   // pinned double buffer through which pageable caller memory is staged (msm_host_on)

@@ -205,6 +205,113 @@ class CachedBases:
             self._h = None
 
 
+FFT_KINDS = {"fft_nn": 0, "fft_nr": 1, "ifft_nn": 2, "ifft_rn": 3,
+             "coset_fft_nn": 4, "coset_fft_nr": 5, "coset_ifft_nn": 6, "coset_ifft_rn": 7}
+FFT_FIELDS = {"bls12_381": 0, "bn254_snarks": 1, "pallas": 2, "vesta": 3}
+
+
+class FFTError(ValueError):
+    """A non-zero status of the FFT entries: 2 too many values, 3 size not a power of two, 4 omega not of the domain's order,
+    5 bad argument (the numbering of the reference's FFTStatus for 1..3)."""
+
+    def __init__(self, status: int, what: str):
+        super().__init__(f"{what}: status {status}")
+        self.status = status
+
+
+def _fft_field_id(curve) -> int:
+    if isinstance(curve, int):
+        return curve
+    if isinstance(curve, CurveParams):
+        curve = curve.name
+    if curve in FFT_FIELDS:
+        return FFT_FIELDS[curve]
+    return _curve(curve).curve_id
+
+
+def _fr_struct(x) -> bytes:
+    """An Fr struct (Montgomery, 4 x u64): 32 bytes as given, or an int already in Montgomery form."""
+    if isinstance(x, int):
+        return x.to_bytes(32, "little")
+    b = bytes(memoryview(x).cast("B"))
+    if len(b) != 32:
+        raise ValueError("an Fr struct is 32 bytes")
+    return b
+
+
+class FFTDomain:
+    """The reference's FrFFT_Descriptor (constantine/math/polynomials/fft_fields.nim) on the device: the Fr of `curve` (curve id
+    0..3 or its name), order 2^log_order, generator `omega` (32-byte Fr struct, Montgomery form) of exactly that order. One domain
+    serves every power-of-two length n <= 2^log_order with omega^(2^log_order / n). Values are reduced Montgomery residues: bytes
+    of batch * n * 32, or numpy uint64[batch * n, 4]; results come back in the same type. `batch` transforms lie back to back."""
+
+    def __init__(self, curve, omega, log_order: int):
+        st = ctypes.c_int(0)
+        self.field_id, self.log_order = _fft_field_id(curve), log_order
+        self._h = _lib.load().ctt_b200_fft_domain_new(self.field_id, _fr_struct(omega), log_order, ctypes.byref(st))
+        if not self._h:
+            raise FFTError(st.value, "ctt_b200_fft_domain_new")
+
+    def _run(self, kind: str, vals, batch: int, shift):
+        lib = _lib.load()
+        sh = _fr_struct(shift) if shift is not None else None
+        is_np = type(vals).__module__ == "numpy"
+        if is_np:
+            # the caller's array is read in place and the result written straight into a new array: no intermediate copies
+            import numpy as np
+            a = np.ascontiguousarray(vals, dtype=np.uint64).reshape(-1, 4)
+            out = np.empty_like(a)
+            src, dst, total = a.ctypes.data, out.ctypes.data, len(a)
+        else:
+            src = _buf(vals)
+            total = len(src) // 32
+            out = ctypes.create_string_buffer(max(1, 32 * total))
+            dst = out
+        if batch < 1 or total % batch:
+            raise ValueError("the values are not batch transforms of one length")
+        rc = lib.ctt_b200_fft(self._h, FFT_KINDS[kind], dst, src if total else dst, total // batch, batch, sh)
+        if rc != 0:
+            raise FFTError(rc, kind)
+        return out if is_np else out.raw[:32 * total]
+
+    def _run_device(self, kind: str, d_out: int, d_in: int, n: int, batch: int, shift):
+        sh = _fr_struct(shift) if shift is not None else None
+        rc = _lib.load().ctt_b200_fft_device(self._h, FFT_KINDS[kind], d_out, d_in, n, batch, sh)
+        if rc != 0:
+            raise FFTError(rc, kind + "_device")
+
+    def fft_nn(self, vals, batch=1): return self._run("fft_nn", vals, batch, None)
+    def fft_nr(self, vals, batch=1): return self._run("fft_nr", vals, batch, None)
+    def ifft_nn(self, vals, batch=1): return self._run("ifft_nn", vals, batch, None)
+    def ifft_rn(self, vals, batch=1): return self._run("ifft_rn", vals, batch, None)
+    def coset_fft_nn(self, vals, shift, batch=1): return self._run("coset_fft_nn", vals, batch, shift)
+    def coset_fft_nr(self, vals, shift, batch=1): return self._run("coset_fft_nr", vals, batch, shift)
+    def coset_ifft_nn(self, vals, shift, batch=1): return self._run("coset_ifft_nn", vals, batch, shift)
+    def coset_ifft_rn(self, vals, shift, batch=1): return self._run("coset_ifft_rn", vals, batch, shift)
+
+    # device pointers (e.g. a torch tensor's data_ptr()); the stream contract of ctt_b200_fft_device
+    def fft_nn_device(self, d_out, d_in, n, batch=1): self._run_device("fft_nn", d_out, d_in, n, batch, None)
+    def fft_nr_device(self, d_out, d_in, n, batch=1): self._run_device("fft_nr", d_out, d_in, n, batch, None)
+    def ifft_nn_device(self, d_out, d_in, n, batch=1): self._run_device("ifft_nn", d_out, d_in, n, batch, None)
+    def ifft_rn_device(self, d_out, d_in, n, batch=1): self._run_device("ifft_rn", d_out, d_in, n, batch, None)
+    def coset_fft_nn_device(self, d_out, d_in, n, shift, batch=1): self._run_device("coset_fft_nn", d_out, d_in, n, batch, shift)
+    def coset_fft_nr_device(self, d_out, d_in, n, shift, batch=1): self._run_device("coset_fft_nr", d_out, d_in, n, batch, shift)
+    def coset_ifft_nn_device(self, d_out, d_in, n, shift, batch=1): self._run_device("coset_ifft_nn", d_out, d_in, n, batch, shift)
+    def coset_ifft_rn_device(self, d_out, d_in, n, shift, batch=1): self._run_device("coset_ifft_rn", d_out, d_in, n, batch, shift)
+
+    @staticmethod
+    def last_timing() -> dict:
+        """The calling thread's last FFT call (ms): upload, kernels and copy back (device entry: kernels only)."""
+        v = [ctypes.c_float() for _ in range(3)]
+        _lib.load().ctt_b200_fft_last_timing(*[ctypes.byref(x) for x in v])
+        return dict(zip(("ms_h2d", "ms_kernels", "ms_d2h"), (x.value for x in v)))
+
+    def free(self):
+        if self._h:
+            _lib.load().ctt_b200_fft_domain_free(self._h)
+            self._h = None
+
+
 def msm_batch(curve, coefs, points, batch: int, length: int, out=OUT_JAC, coef_kind="big", shared_points=False) -> list:
     """r[m] = sum_i coefs[m*length + i] * points[(0 if shared_points else m*length) + i] for m < batch, host buffers, one
     engine pass (ctt_b200_msm_batch_host). Returns the list of result structs."""
