@@ -96,6 +96,14 @@ def load():
         fn = getattr(lib, nm)
         fn.argtypes = [vp, sz, vp, sz]
         fn.restype = ctypes.c_ubyte
+    lib.ctt_eth_evm_bn254_ecpairingcheck.argtypes = [vp, sz, vp, sz]
+    lib.ctt_eth_evm_bn254_ecpairingcheck.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_evm_bn254_ecpairingcheck_batch.argtypes = [vp, vp, vp, sz, vp, sz]
+    lib.ctt_b200_eth_evm_bn254_ecpairingcheck_batch.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_evm_bn254_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 4
+    lib.ctt_b200_eth_evm_bn254_last_timing.restype = None
+    lib.ctt_b200_test_bn254_pairing.argtypes = [vp, vp, sz, vp]
+    lib.ctt_b200_test_bn254_pairing.restype = ci
     lib.ctt_b200_eth_kzg_context_new.argtypes = [vp]
     lib.ctt_b200_eth_kzg_context_new.restype = vp
     lib.ctt_b200_eth_kzg_context_new_compressed.argtypes = [vp, ctypes.POINTER(ci)]

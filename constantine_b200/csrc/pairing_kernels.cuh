@@ -1,5 +1,6 @@
-// BLS12-381 optimal ate pairing on the device: Fp6 / Fp12 over the device Fp2, the Miller loop with T in homogeneous projective
-// coordinates and sparse line products, the tree product of the per-pair values and the final exponentiation.
+// BLS12-381 optimal ate pairing on the device: Fp6 / Fp12 over the device Fp2 (the shared tower of tower.cuh), the Miller loop with
+// T in homogeneous projective coordinates and sparse line products, the tree product of the per-pair values and the final
+// exponentiation.
 //
 // Tower: the one of host_pairing.hpp (Fp6 = Fp2[v] / (v^3 - xi), xi = 1 + i, Fp12 = Fp6[w] / (w^2 - v)), so the GT bytes compare
 // directly with the host. Lines are the host's, scaled by factors in Fp2, which the final exponentiation removes.
@@ -10,8 +11,7 @@
 // therefore e(P, Q)^3; k = 3 is coprime to r, so e^3 = 1 exactly when e = 1.
 // Not constant time: every input of a verification is public.
 #pragma once
-#include "ec.cuh"
-#include "field_inv.cuh"
+#include "tower.cuh"
 #include "bls_constants.cuh"
 
 namespace b200 {
@@ -22,127 +22,26 @@ using Fq2 = Fp2<Bls12381Fp>;
 constexpr unsigned long long ATE_X = 0xd201000000010000ull;   // |x|, x = -0xd201000000010000
 constexpr int GT_WORDS = 12 * Fq::WORDS;                     // 144
 
-B200_DEV Fq2 fq2_const(const uint32_t* tab, int idx) {
-  Fq2 r;
-#pragma unroll
-  for (int k = 0; k < Fq2::WORDS; k++) r.set_word(k, tab[idx * Fq2::WORDS + k]);
-  return r;
-}
+B200_DEV Fq2 fq2_const(const uint32_t* tab, int idx) { return b200::fq2_const<Bls12381Fp>(tab, idx); }
 B200_DEV Fq2 mul_xi(const Fq2& a) { Fq2 r; r.c0 = a.c0 - a.c1; r.c1 = a.c0 + a.c1; return r; }
-B200_DEV Fq2 conj2(const Fq2& a) { Fq2 r; r.c0 = a.c0; r.c1 = a.c1.neg(); return r; }
+B200_DEV Fq2 conj2(const Fq2& a) { return fq2_conj(a); }
 B200_DEV Fq2 scale(const Fq2& a, const Fq& s) { Fq2 r; r.c0 = a.c0 * s; r.c1 = a.c1 * s; return r; }
 
-struct Fq6 {
-  Fq2 c0, c1, c2;
-  B200_DEV static Fq6 zero() { Fq6 r; r.c0 = Fq2::zero(); r.c1 = Fq2::zero(); r.c2 = Fq2::zero(); return r; }
-  B200_DEV static Fq6 one() { Fq6 r = zero(); r.c0 = Fq2::one(); return r; }
-  B200_DEV Fq6 operator+(const Fq6& b) const { Fq6 r; r.c0 = c0 + b.c0; r.c1 = c1 + b.c1; r.c2 = c2 + b.c2; return r; }
-  B200_DEV Fq6 operator-(const Fq6& b) const { Fq6 r; r.c0 = c0 - b.c0; r.c1 = c1 - b.c1; r.c2 = c2 - b.c2; return r; }
-  B200_DEV Fq6 neg() const { Fq6 r; r.c0 = c0.neg(); r.c1 = c1.neg(); r.c2 = c2.neg(); return r; }
-  B200_DEV Fq6 mul_by_v() const { Fq6 r; r.c0 = mul_xi(c2); r.c1 = c0; r.c2 = c1; return r; }
-  B200_DEV bool is_one() const { return c0 == Fq2::one() && c1.is_zero() && c2.is_zero(); }
+// the tower of tower.cuh with xi = 1 + i
+struct Tower {
+  using Fq2 = bls::Fq2;
+  static B200_DEV Fq2 mul_xi(const Fq2& a) { return bls::mul_xi(a); }
+  static B200_DEV Fq2 gamma(int k) { return fq2_const(PAIR_FROB, k); }
 };
+using Fq6 = Fp6T<Tower>;
+using Fq12 = Fp12T<Tower>;
 
-// Karatsuba over the three coefficients, v^3 = xi (host_pairing.hpp Fp6::operator*)
-__device__ __noinline__ Fq6 fq6_mul(const Fq6& a, const Fq6& b) {
-  const Fq2 t0 = a.c0 * b.c0, t1 = a.c1 * b.c1, t2 = a.c2 * b.c2;
-  Fq6 r;
-  r.c0 = t0 + mul_xi((a.c1 + a.c2) * (b.c1 + b.c2) - t1 - t2);
-  r.c1 = (a.c0 + a.c1) * (b.c0 + b.c1) - t0 - t1 + mul_xi(t2);
-  r.c2 = (a.c0 + a.c2) * (b.c0 + b.c2) - t0 - t2 + t1;
-  return r;
-}
-// a * (b0 + b1 v)
-__device__ __noinline__ Fq6 fq6_mul_01(const Fq6& a, const Fq2& b0, const Fq2& b1) {
-  const Fq2 t0 = a.c0 * b0, t1 = a.c1 * b1;
-  Fq6 r;
-  r.c0 = t0 + mul_xi((a.c1 + a.c2) * b1 - t1);
-  r.c1 = (a.c0 + a.c1) * (b0 + b1) - t0 - t1;
-  r.c2 = (a.c0 + a.c2) * b0 - t0 + t1;
-  return r;
-}
-// a * (b1 v)
-B200_DEV Fq6 fq6_mul_1(const Fq6& a, const Fq2& b1) {
-  Fq6 r;
-  r.c0 = mul_xi(a.c2 * b1);
-  r.c1 = a.c0 * b1;
-  r.c2 = a.c1 * b1;
-  return r;
-}
-__device__ __noinline__ Fq6 fq6_inv(const Fq6& a) {
-  const Fq2 A = a.c0.sqr() - mul_xi(a.c1 * a.c2), B = mul_xi(a.c2.sqr()) - a.c0 * a.c1, C = a.c1.sqr() - a.c0 * a.c2;
-  const Fq2 F = fe_inverse(a.c0 * A + mul_xi(a.c2 * B + a.c1 * C));
-  Fq6 r; r.c0 = A * F; r.c1 = B * F; r.c2 = C * F;
-  return r;
-}
-
-struct Fq12 {
-  Fq6 c0, c1;
-  B200_DEV static Fq12 one() { Fq12 r; r.c0 = Fq6::one(); r.c1 = Fq6::zero(); return r; }
-  B200_DEV Fq12 conj() const { Fq12 r; r.c0 = c0; r.c1 = c1.neg(); return r; }
-  B200_DEV bool is_one() const { return c0.is_one() && c1.c0.is_zero() && c1.c1.is_zero() && c1.c2.is_zero(); }
-};
-
-__device__ __noinline__ Fq12 fq12_mul(const Fq12& a, const Fq12& b) {   // w^2 = v
-  const Fq6 t0 = fq6_mul(a.c0, b.c0), t1 = fq6_mul(a.c1, b.c1);
-  Fq12 r;
-  r.c0 = t0 + t1.mul_by_v();
-  r.c1 = fq6_mul(a.c0 + a.c1, b.c0 + b.c1) - t0 - t1;
-  return r;
-}
-// (c0 + c1 w)^2 = c0^2 + c1^2 v + 2 c0 c1 w with two Fp6 products
-__device__ __noinline__ Fq12 fq12_sqr(const Fq12& a) {
-  const Fq6 t = fq6_mul(a.c0, a.c1);
-  Fq12 r;
-  r.c0 = fq6_mul(a.c0 + a.c1, a.c0 + a.c1.mul_by_v()) - t - t.mul_by_v();
-  r.c1 = t + t;
-  return r;
-}
 // f * l for the sparse line l = a + b w^2 + c w^3 = (a + b v) + (c v) w
 __device__ __noinline__ Fq12 fq12_mul_line(const Fq12& f, const Fq2& a, const Fq2& b, const Fq2& c) {
   const Fq6 t0 = fq6_mul_01(f.c0, a, b), t1 = fq6_mul_1(f.c1, c);
   Fq12 r;
   r.c0 = t0 + t1.mul_by_v();
   r.c1 = fq6_mul_01(f.c0 + f.c1, a, b + c) - t0 - t1;
-  return r;
-}
-__device__ __noinline__ Fq12 fq12_inv(const Fq12& a) {
-  const Fq6 t = fq6_inv(fq6_mul(a.c0, a.c0) - fq6_mul(a.c1, a.c1).mul_by_v());
-  Fq12 r; r.c0 = fq6_mul(a.c0, t); r.c1 = fq6_mul(a.c1, t).neg();
-  return r;
-}
-// f^p: the coefficient of w^k (c0 = w^0, w^2, w^4; c1 = w^1, w^3, w^5) is conjugated and multiplied by gamma_k
-__device__ __noinline__ Fq12 fq12_frob(const Fq12& a) {
-  Fq12 r;
-  r.c0.c0 = conj2(a.c0.c0);
-  r.c0.c1 = conj2(a.c0.c1) * fq2_const(PAIR_FROB, 1);
-  r.c0.c2 = conj2(a.c0.c2) * fq2_const(PAIR_FROB, 3);
-  r.c1.c0 = conj2(a.c1.c0) * fq2_const(PAIR_FROB, 0);
-  r.c1.c1 = conj2(a.c1.c1) * fq2_const(PAIR_FROB, 2);
-  r.c1.c2 = conj2(a.c1.c2) * fq2_const(PAIR_FROB, 4);
-  return r;
-}
-// a^2 for a in the cyclotomic subgroup (Granger-Scott, "Faster squaring in the cyclotomic subgroup of sixth degree extensions",
-// PKC 2010): three Fp4 squarings. Coefficients by powers of w: z0 = c0.c0, z4 = c0.c1, z3 = c0.c2, z2 = c1.c0, z1 = c1.c1, z5 = c1.c2.
-B200_DEV void fp4_sqr(Fq2& t0, Fq2& t1, const Fq2& a, const Fq2& b) {   // (a + b y)^2 with y^2 = xi
-  const Fq2 t = a * b;
-  t0 = (a + b) * (mul_xi(b) + a) - t - mul_xi(t);
-  t1 = t + t;
-}
-__device__ __noinline__ Fq12 fq12_cyclotomic_sqr(const Fq12& a) {
-  Fq2 t0, t1, t2, t3, t4, t5;
-  fp4_sqr(t0, t1, a.c0.c0, a.c1.c1);
-  fp4_sqr(t2, t3, a.c1.c0, a.c0.c2);
-  fp4_sqr(t4, t5, a.c0.c1, a.c1.c2);
-  Fq12 r;
-  Fq2 z;
-  z = t0 - a.c0.c0; r.c0.c0 = z + z + t0;          // 3 t0 - 2 z0
-  z = t1 + a.c1.c1; r.c1.c1 = z + z + t1;          // 3 t1 + 2 z1
-  const Fq2 xt5 = mul_xi(t5);
-  z = xt5 + a.c1.c0; r.c1.c0 = z + z + xt5;        // 3 xi t5 + 2 z2
-  z = t4 - a.c0.c2; r.c0.c2 = z + z + t4;          // 3 t4 - 2 z3
-  z = t2 - a.c0.c1; r.c0.c1 = z + z + t2;          // 3 t2 - 2 z4
-  z = t3 + a.c1.c2; r.c1.c2 = z + z + t3;          // 3 t3 + 2 z5
   return r;
 }
 // a^x for a in the cyclotomic subgroup (x < 0: the conjugate of a^|x|)
@@ -228,18 +127,7 @@ B200_DEV Fq12 miller_loop(const Aff<Fq>& P, const Aff<Fq2>& Q) {
   return f.conj();
 }
 
-B200_DEV void store_fq12(uint32_t* dst, const Fq12& f) {
-  const Fq2* c[6] = {&f.c0.c0, &f.c0.c1, &f.c0.c2, &f.c1.c0, &f.c1.c1, &f.c1.c2};
-#pragma unroll
-  for (int k = 0; k < 6; k++) store_words(dst + k * Fq2::WORDS, *c[k]);
-}
-B200_DEV Fq12 load_fq12(const uint32_t* src) {
-  Fq12 f;
-  Fq2* c[6] = {&f.c0.c0, &f.c0.c1, &f.c0.c2, &f.c1.c0, &f.c1.c1, &f.c1.c2};
-#pragma unroll
-  for (int k = 0; k < 6; k++) load_words_rw(*c[k], src + k * Fq2::WORDS);
-  return f;
-}
+B200_DEV Fq12 load_fq12(const uint32_t* src) { return b200::load_fq12<Tower>(src); }
 
 constexpr int PAIR_THREADS = 64;
 

@@ -407,6 +407,44 @@ def eth_evm_bls12381_g2msm(inputs: bytes, out_len: int = 256):
     return EVM_STATUS[st], r.raw
 
 
+def eth_evm_bn254_ecpairingcheck(inputs: bytes, out_len: int = 32):
+    """EIP-197 ecPairing on BN254 through ctt_eth_evm_bn254_ecpairingcheck (reference constantine/ethereum_evm_precompiles.nim:543-626):
+    k x 192 bytes of (P.x, P.y, Q.x_im, Q.x_re, Q.y_im, Q.y_re), 32-byte big-endian each. Returns (status name, output bytes), the
+    output 32 bytes holding 0 or 1. A pair with an infinity point contributes 1 and the other pairs still count (EIP-197)."""
+    r = ctypes.create_string_buffer(max(out_len, 1))
+    inputs = bytes(inputs)
+    st = _lib.load().ctt_eth_evm_bn254_ecpairingcheck(r, out_len, inputs, len(inputs))
+    return EVM_STATUS[st], r.raw[:out_len]
+
+
+def eth_evm_bn254_ecpairingcheck_batch(calls) -> list:
+    """Many independent ecPairing calls in one pass (ctt_b200_eth_evm_bn254_ecpairingcheck_batch): calls is a sequence of byte
+    strings; returns [(status name, 32 output bytes)] in the same order, as the single entry gives them per call."""
+    calls = [bytes(c) for c in calls]
+    k = len(calls)
+    if k == 0:
+        return []
+    offsets = (ctypes.c_size_t * (k + 1))()
+    for i, c in enumerate(calls):
+        offsets[i + 1] = offsets[i] + len(c)
+    data = b"".join(calls) or b"\0"
+    r = ctypes.create_string_buffer(32 * k)
+    statuses = ctypes.create_string_buffer(k)
+    st = _lib.load().ctt_b200_eth_evm_bn254_ecpairingcheck_batch(r, statuses, data, offsets[k], offsets, k)
+    if st != 0:
+        raise ValueError(EVM_STATUS[st])
+    raw = r.raw
+    return [(EVM_STATUS[statuses.raw[i]], raw[32 * i:32 * i + 32]) for i in range(k)]
+
+
+def eth_evm_bn254_last_timing() -> dict:
+    """Host checks and packing, device decoding, Miller loops, and products with final exponentiations (ms) of the calling thread's
+    last ecPairing call."""
+    v = [ctypes.c_float(0) for _ in range(4)]
+    _lib.load().ctt_b200_eth_evm_bn254_last_timing(*[ctypes.byref(x) for x in v])
+    return dict(zip(("ms_host", "ms_decode", "ms_miller", "ms_final"), (x.value for x in v)))
+
+
 class CtSpan(ctypes.Structure):
     """ctt_span: {byte* data; size_t len} (reference include/constantine/protocols/ethereum_bls_signatures.h:64)."""
     _fields_ = [("data", ctypes.c_void_p), ("len", ctypes.c_size_t)]
