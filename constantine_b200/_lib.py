@@ -102,6 +102,18 @@ def load():
     lib.ctt_b200_eth_evm_bn254_ecpairingcheck_batch.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_evm_bn254_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 4
     lib.ctt_b200_eth_evm_bn254_last_timing.restype = None
+    for nm in ("ctt_eth_evm_bls12381_pairingcheck", "ctt_eth_evm_bls12381_map_fp_to_g1", "ctt_eth_evm_bls12381_map_fp2_to_g2"):
+        fn = getattr(lib, nm)
+        fn.argtypes = [vp, sz, vp, sz]
+        fn.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_evm_bls12381_pairingcheck_batch.argtypes = [vp, vp, vp, sz, vp, sz]
+    lib.ctt_b200_eth_evm_bls12381_pairingcheck_batch.restype = ctypes.c_ubyte
+    for nm in ("ctt_b200_eth_evm_bls12381_map_fp_to_g1_batch", "ctt_b200_eth_evm_bls12381_map_fp2_to_g2_batch"):
+        fn = getattr(lib, nm)
+        fn.argtypes = [vp, vp, vp, sz]
+        fn.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_evm_bls12381_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 5
+    lib.ctt_b200_eth_evm_bls12381_last_timing.restype = None
     lib.ctt_b200_test_bn254_pairing.argtypes = [vp, vp, sz, vp]
     lib.ctt_b200_test_bn254_pairing.restype = ci
     lib.ctt_b200_eth_kzg_context_new.argtypes = [vp]

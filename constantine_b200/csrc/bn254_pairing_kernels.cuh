@@ -244,7 +244,7 @@ __device__ __noinline__ uint8_t decode_pair(const uint8_t* src, Aff<Fq>& P, Aff<
 }
 
 constexpr int DECODE_THREADS = 128;
-constexpr int PAIR_THREADS = 64;
+constexpr int PAIR_THREADS = PAIRING_THREADS;
 
 // src: n x 192 bytes; g1: n affine G1 points (16 words), g2: n affine G2 points (32 words); status: n ctt_evm_status values
 __global__ void __launch_bounds__(DECODE_THREADS) k_bn_decode(const uint8_t* __restrict__ src, size_t n, uint32_t* g1, uint32_t* g2,
@@ -269,28 +269,9 @@ __global__ void __launch_bounds__(PAIR_THREADS) k_bn_miller(const uint32_t* g1, 
   store_fq12(f + i * GT_WORDS, miller_loop(P, Q));
 }
 
-// One level of the products of the calls, in place: call c owns the values begin[c] .. begin[c + 1] - 1 and call_of[i] is the call of
-// value i. At level `stride` = 2^l the value at offset j of its call, j a multiple of 2 stride, takes the product with the value at
-// j + stride when that exists; after ceil(log2(longest call)) levels each call's product sits at offset 0.
-__global__ void __launch_bounds__(PAIR_THREADS) k_bn_fold(uint32_t* f, const size_t* call_of, const size_t* begin, size_t n,
-                                                          size_t stride) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const size_t c = call_of[i], j = i - begin[c];
-  if (j % (2 * stride) != 0 || j + stride >= begin[c + 1] - begin[c]) return;
-  store_fq12(f + i * GT_WORDS, fq12_mul(load_fq12<Tower>(f + i * GT_WORDS), load_fq12<Tower>(f + (i + stride) * GT_WORDS)));
-}
-
-// One thread per call (each has at least one value): ok[c] = (final_exponentiation(f[begin[c]]) == 1); gt (if not null) receives
-// the GT values, ncalls x 96 words
-__global__ void __launch_bounds__(PAIR_THREADS) k_bn_final_exp(const uint32_t* f, const size_t* begin, size_t ncalls, uint8_t* ok,
-                                                               uint32_t* gt) {
-  const size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= ncalls) return;
-  const Fq12 r = final_exponentiation(load_fq12<Tower>(f + begin[c] * GT_WORDS));
-  ok[c] = r.is_one() ? 1 : 0;
-  if (gt) store_fq12(gt + c * GT_WORDS, r);
-}
+struct FinalExp {   // for k_pairing_final_exp (tower.cuh)
+  static B200_DEV Fq12 apply(const Fq12& f) { return final_exponentiation(f); }
+};
 
 }  // namespace bn
 }  // namespace b200

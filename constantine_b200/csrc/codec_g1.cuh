@@ -85,6 +85,19 @@ static __device__ __noinline__ bool g1_in_subgroup(const G1Fp& x, const G1Fp& y)
   return !t.is_inf() && (beta * x) * t.zz == t.x && y * t.zzz == t.y.neg();
 }
 
+// a^((p + 1) / 4): a square root of a when a is a square (p = 3 mod 4); the caller checks it by squaring
+static __device__ __noinline__ G1Fp sqrt_candidate(const G1Fp& a) {
+  uint32_t e[12];
+  p_words(e, 1, 2);                                   // (p + 1) / 4
+  G1Fp y = G1Fp::one();
+#pragma unroll 1
+  for (int b = 380; b >= 0; b--) {
+    y = y.sqr();
+    if ((e[b >> 5] >> (b & 31)) & 1u) y = y * a;
+  }
+  return y;
+}
+
 // The G1 decoder: xw the canonical x (12 little-endian words, < p), sign the 0x20 flag. y = (x^3 + 4)^((p + 1) / 4), checked by
 // squaring (p = 3 mod 4); the root whose lexicographic sign matches the flag; then the subgroup test. Returns CODEC_OK with (x, y) set
 // (Montgomery), CODEC_NOT_ON_CURVE or CODEC_NOT_IN_SUBGROUP.
@@ -93,14 +106,7 @@ static __device__ __noinline__ int g1_decode(const uint32_t* xw, bool sign, G1Fp
   G1Fp four = G1Fp::one().dbl();
   four = four.dbl();
   const G1Fp rhs = x.sqr() * x + four;
-  uint32_t e[12];
-  p_words(e, 1, 2);                                   // (p + 1) / 4
-  G1Fp y = G1Fp::one();
-#pragma unroll 1
-  for (int b = 380; b >= 0; b--) {
-    y = y.sqr();
-    if ((e[b >> 5] >> (b & 31)) & 1u) y = y * rhs;
-  }
+  G1Fp y = sqrt_candidate(rhs);
   if (!(y.sqr() == rhs)) return CODEC_NOT_ON_CURVE;
   if (lexicographically_largest(y) != sign) y = y.neg();
   if (!g1_in_subgroup(x, y)) return CODEC_NOT_IN_SUBGROUP;

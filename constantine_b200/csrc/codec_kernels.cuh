@@ -10,6 +10,7 @@
 // The point is written as the affine Montgomery struct (ctt_eth_bls_pubkey / ctt_eth_bls_signature) when the status is 0, as zeros
 // otherwise. Included by eth_bls.cu only (it pulls in the hash-to-G2 kernels for fq2_sqrt and psi).
 // Not constant time: every input is public.
+// Its functions and kernels are static: eth_bls.cu and evm_bls12381_precompiles.cu both include it.
 #pragma once
 #include "h2c_kernels.cuh"
 #include "codec_g1.cuh"
@@ -50,7 +51,7 @@ B200_DEV bool all_zero(const uint32_t* w) {
 }
 
 // Q = (x, y) affine Montgomery, on the curve: psi(Q) = [u]Q (h2c_kernels.cuh: psi, and mul_by_x = [u])
-__device__ __noinline__ bool g2_in_subgroup(const Fq2& x, const Fq2& y) {
+static __device__ __noinline__ bool g2_in_subgroup(const Fq2& x, const Fq2& y) {
   Xyzz<Fq2> q;
   q.x = x; q.y = y; q.zz = Fq2::one(); q.zzz = Fq2::one();
   const Xyzz<Fq2> t = bls::mul_by_x(q);
@@ -61,7 +62,7 @@ __device__ __noinline__ bool g2_in_subgroup(const Fq2& x, const Fq2& y) {
 // The G2 decoder: c0w, c1w the canonical x.c0 and x.c1 (< p), sign the 0x20 flag. y a square root of x^3 + 4(1 + i) (fq2_sqrt), the
 // root whose sign (y.c1 decides, y.c0 when y.c1 = 0) matches the flag, then the subgroup test. Returns CODEC_OK with (x, y) set,
 // CODEC_NOT_ON_CURVE or CODEC_NOT_IN_SUBGROUP.
-__device__ __noinline__ int g2_decode(const uint32_t* c0w, const uint32_t* c1w, bool sign, Fq2& x_out, Fq2& y_out) {
+static __device__ __noinline__ int g2_decode(const uint32_t* c0w, const uint32_t* c1w, bool sign, Fq2& x_out, Fq2& y_out) {
   Fq2 x, b, y;
   x.c0 = to_mont(c0w);
   x.c1 = to_mont(c1w);
@@ -78,7 +79,7 @@ __device__ __noinline__ int g2_decode(const uint32_t* c0w, const uint32_t* c1w, 
 }
 
 // src: n x 48 bytes; out: n x 96 bytes (affine Montgomery x, y); status: n codec statuses
-__global__ void __launch_bounds__(DECODE_THREADS) k_bls_decode_g1(const uint8_t* __restrict__ src, size_t n, uint32_t* out,
+static __global__ void __launch_bounds__(DECODE_THREADS) k_bls_decode_g1(const uint8_t* __restrict__ src, size_t n, uint32_t* out,
                                                                   uint8_t* status) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -100,7 +101,7 @@ __global__ void __launch_bounds__(DECODE_THREADS) k_bls_decode_g1(const uint8_t*
 }
 
 // src: n x 96 bytes; out: n x 192 bytes (affine Montgomery x.c0, x.c1, y.c0, y.c1); status: n codec statuses
-__global__ void __launch_bounds__(DECODE_THREADS) k_bls_decode_g2(const uint8_t* __restrict__ src, size_t n, uint32_t* out,
+static __global__ void __launch_bounds__(DECODE_THREADS) k_bls_decode_g2(const uint8_t* __restrict__ src, size_t n, uint32_t* out,
                                                                   uint8_t* status) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;

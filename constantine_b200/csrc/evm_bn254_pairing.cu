@@ -78,12 +78,12 @@ static void pairing_device(const uint8_t* wire, const uint8_t* g1, const uint8_t
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaEventRecord(ev[2], s));
   for (size_t stride = 1; stride < longest; stride *= 2) {
-    bn::k_bn_fold<<<blocks(npairs, bn::PAIR_THREADS), bn::PAIR_THREADS, 0, s>>>((uint32_t*)d_f, (const size_t*)d_call,
-                                                                                (const size_t*)d_begin, npairs, stride);
+    k_pairing_fold<bn::Tower><<<blocks(npairs, bn::PAIR_THREADS), bn::PAIR_THREADS, 0, s>>>((uint32_t*)d_f, (const size_t*)d_call,
+                                                                                            (const size_t*)d_begin, npairs, stride);
     B200_CUDA_CHECK(cudaGetLastError());
   }
-  bn::k_bn_final_exp<<<blocks(ncalls, bn::PAIR_THREADS), bn::PAIR_THREADS, 0, s>>>((const uint32_t*)d_f, (const size_t*)d_begin, ncalls,
-                                                                                   (uint8_t*)d_ok, (uint32_t*)d_gt);
+  k_pairing_final_exp<bn::Tower, bn::FinalExp><<<blocks(ncalls, bn::PAIR_THREADS), bn::PAIR_THREADS, 0, s>>>(
+      (const uint32_t*)d_f, (const size_t*)d_begin, ncalls, (uint8_t*)d_ok, (uint32_t*)d_gt);
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaEventRecord(ev[3], s));
   B200_CUDA_CHECK(cudaMemcpyAsync(ok, d_ok, ncalls, cudaMemcpyDeviceToHost, s));

@@ -5,6 +5,7 @@
 //   the 3-isogeny E2' -> E2 (generated: tools/gen_bls_constants.py);
 //   Q0 + Q1 and the cofactor clearing h_eff P = [x^2 - x - 1]P + [x - 1]psi(P) + psi^2(2P) (Budroni-Pintore; RFC appendix G.3);
 //   the affine result, for the Miller loop.
+// Its functions and kernels are static: eth_bls.cu and evm_bls12381_precompiles.cu both include it.
 #pragma once
 #include "pairing_kernels.cuh"
 
@@ -21,7 +22,7 @@ B200_DEV void p_minus_shift(uint32_t e[12], uint32_t sub, int shift) {
   for (int k = 0; k < 12; k++) e[k] = (t[k] >> shift) | (k + 1 < 12 ? t[k + 1] << (32 - shift) : 0u);
 }
 
-__device__ __noinline__ Fq2 fq2_pow(const Fq2& a, const uint32_t e[12]) {
+static __device__ __noinline__ Fq2 fq2_pow(const Fq2& a, const uint32_t e[12]) {
   Fq2 r = Fq2::one();
 #pragma unroll 1
   for (int i = 381; i >= 0; i--) {
@@ -32,7 +33,7 @@ __device__ __noinline__ Fq2 fq2_pow(const Fq2& a, const uint32_t e[12]) {
 }
 
 // A square root of a (Adj and Rodriguez-Henriquez 2012, algorithm 9, as host_pairing.hpp fp2_sqrt); false when a is not a square
-__device__ __noinline__ bool fq2_sqrt(Fq2& out, const Fq2& a) {
+static __device__ __noinline__ bool fq2_sqrt(Fq2& out, const Fq2& a) {
   uint32_t e[12];
   p_minus_shift(e, 3, 2);                       // (p - 3) / 4
   const Fq2 a1 = fq2_pow(a, e);
@@ -84,7 +85,7 @@ B200_DEV Fq2 horner(int first, int count, const Fq2& x) {
 }
 
 // SSWU(u) on E2', then the isogeny to E2; affine
-__device__ __noinline__ Aff<Fq2> map_to_curve(const Fq2& u) {
+static __device__ __noinline__ Aff<Fq2> map_to_curve(const Fq2& u) {
   const Fq2 A = fq2_const(H2C_SSWU, 0), B = fq2_const(H2C_SSWU, 1), Z = fq2_const(H2C_SSWU, 2);
   const Fq2 zu2 = Z * u.sqr();
   const Fq2 den = zu2.sqr() + zu2;
@@ -117,7 +118,7 @@ B200_DEV Xyzz<Fq2> psi(const Xyzz<Fq2>& p) {
 B200_DEV Xyzz<Fq2> xyzz_neg(Xyzz<Fq2> p) { p.y = p.y.neg(); return p; }
 
 // [x]P, x = -|x|
-__device__ __noinline__ Xyzz<Fq2> mul_by_x(const Xyzz<Fq2>& p) {
+static __device__ __noinline__ Xyzz<Fq2> mul_by_x(const Xyzz<Fq2>& p) {
   Xyzz<Fq2> acc = p;
 #pragma unroll 1
   for (int bit = 62; bit >= 0; bit--) {
@@ -128,7 +129,7 @@ __device__ __noinline__ Xyzz<Fq2> mul_by_x(const Xyzz<Fq2>& p) {
 }
 
 // RFC 9380 appendix G.3, clear_cofactor_bls12381_g2
-__device__ __noinline__ Xyzz<Fq2> clear_cofactor(const Xyzz<Fq2>& p) {
+static __device__ __noinline__ Xyzz<Fq2> clear_cofactor(const Xyzz<Fq2>& p) {
   const Xyzz<Fq2> t1 = mul_by_x(p);
   Xyzz<Fq2> t2 = psi(p);
   Xyzz<Fq2> t3 = p;
@@ -146,7 +147,7 @@ __device__ __noinline__ Xyzz<Fq2> clear_cofactor(const Xyzz<Fq2>& p) {
 constexpr int H2C_THREADS = 64;
 
 // uniform: n x 256 bytes of expand_message_xmd; out: n affine G2 points (ABI layout, infinity (0, 0))
-__global__ void __launch_bounds__(H2C_THREADS) k_bls_hash_to_g2(const uint8_t* uniform, size_t n, uint32_t* out) {
+static __global__ void __launch_bounds__(H2C_THREADS) k_bls_hash_to_g2(const uint8_t* uniform, size_t n, uint32_t* out) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint8_t* s = uniform + 256 * i;

@@ -10,6 +10,7 @@
 // curves", 2020): five exponentiations by |x| with cyclotomic squarings (Granger-Scott), a few Frobenius maps. The result is
 // therefore e(P, Q)^3; k = 3 is coprime to r, so e^3 = 1 exactly when e = 1.
 // Not constant time: every input of a verification is public.
+// Its functions and kernels are static: eth_bls.cu and evm_bls12381_precompiles.cu both include it.
 #pragma once
 #include "tower.cuh"
 #include "bls_constants.cuh"
@@ -37,7 +38,7 @@ using Fq6 = Fp6T<Tower>;
 using Fq12 = Fp12T<Tower>;
 
 // f * l for the sparse line l = a + b w^2 + c w^3 = (a + b v) + (c v) w
-__device__ __noinline__ Fq12 fq12_mul_line(const Fq12& f, const Fq2& a, const Fq2& b, const Fq2& c) {
+static __device__ __noinline__ Fq12 fq12_mul_line(const Fq12& f, const Fq2& a, const Fq2& b, const Fq2& c) {
   const Fq6 t0 = fq6_mul_01(f.c0, a, b), t1 = fq6_mul_1(f.c1, c);
   Fq12 r;
   r.c0 = t0 + t1.mul_by_v();
@@ -45,7 +46,7 @@ __device__ __noinline__ Fq12 fq12_mul_line(const Fq12& f, const Fq2& a, const Fq
   return r;
 }
 // a^x for a in the cyclotomic subgroup (x < 0: the conjugate of a^|x|)
-__device__ __noinline__ Fq12 cyclotomic_exp_x(const Fq12& a) {
+static __device__ __noinline__ Fq12 cyclotomic_exp_x(const Fq12& a) {
   Fq12 r = a;
 #pragma unroll 1
   for (int bit = 62; bit >= 0; bit--) {
@@ -56,7 +57,7 @@ __device__ __noinline__ Fq12 cyclotomic_exp_x(const Fq12& a) {
 }
 
 // f^(3 (p^12 - 1) / r)
-__device__ __noinline__ Fq12 final_exponentiation(const Fq12& f) {
+static __device__ __noinline__ Fq12 final_exponentiation(const Fq12& f) {
   Fq12 g = fq12_mul(f.conj(), fq12_inv(f));               // f^(p^6 - 1)
   g = fq12_mul(fq12_frob(fq12_frob(g)), g);               // ^(p^2 + 1): now in the cyclotomic subgroup
   Fq12 a = fq12_mul(cyclotomic_exp_x(g), g.conj());        // g^(x - 1)
@@ -66,6 +67,10 @@ __device__ __noinline__ Fq12 final_exponentiation(const Fq12& f) {
   c = fq12_mul(c, b.conj());                               // ^(x^2 + p^2 - 1)
   return fq12_mul(c, fq12_mul(fq12_cyclotomic_sqr(g), g)); // * g^3
 }
+
+struct FinalExp {   // for k_pairing_final_exp (tower.cuh)
+  static B200_DEV Fq12 apply(const Fq12& f) { return final_exponentiation(f); }
+};
 
 // ---- Miller loop ---------------------------------------------------------------------------------------------------------------
 // T = (X : Y : Z) homogeneous projective on the twist E': y^2 = x^3 + 4 xi. P affine in G1, Q affine in G2, both finite.
@@ -77,7 +82,7 @@ __device__ __noinline__ Fq12 final_exponentiation(const Fq12& f) {
 // and T + Q = (d H : t (F - H) - Y G : Z G) with F = d^2 X, G = d^3, H = t^2 Z + G - 2F.
 struct Proj2 { Fq2 x, y, z; };
 
-__device__ __noinline__ Fq12 miller_dbl(Proj2& T, const Fq12& f, const Fq& xP, const Fq& yP) {
+static __device__ __noinline__ Fq12 miller_dbl(Proj2& T, const Fq12& f, const Fq& xP, const Fq& yP) {
   const Fq2 XX = T.x.sqr(), YY = T.y.sqr(), YZ = T.y * T.z;
   const Fq2 XXX = XX * T.x, YYZ = YY * T.z;
   const Fq2 la = XXX + XXX + XXX - YYZ - YYZ;                          // 3 X^3 - 2 Y^2 Z
@@ -97,7 +102,7 @@ __device__ __noinline__ Fq12 miller_dbl(Proj2& T, const Fq12& f, const Fq& xP, c
   return fq12_mul_line(fq12_sqr(f), la, nb, lc + lc);
 }
 
-__device__ __noinline__ Fq12 miller_add(Proj2& T, const Fq12& f, const Fq2& xQ, const Fq2& yQ, const Fq& xP, const Fq& yP) {
+static __device__ __noinline__ Fq12 miller_add(Proj2& T, const Fq12& f, const Fq2& xQ, const Fq2& yQ, const Fq& xP, const Fq& yP) {
   const Fq2 t = T.y - yQ * T.z, d = T.x - xQ * T.z;
   const Fq2 la = t * xQ - d * yQ;
   const Fq2 nb = scale(t, xP).neg();
@@ -132,7 +137,7 @@ B200_DEV Fq12 load_fq12(const uint32_t* src) { return b200::load_fq12<Tower>(src
 constexpr int PAIR_THREADS = 64;
 
 // One pair per thread: f_i = miller_loop(P_i, Q_i). g1: n affine G1 points, g2: n affine G2 points (ABI layout), f: n x 144 words.
-__global__ void __launch_bounds__(PAIR_THREADS) k_bls_miller(const uint32_t* g1, const uint32_t* g2, size_t n, uint32_t* f) {
+static __global__ void __launch_bounds__(PAIR_THREADS) k_bls_miller(const uint32_t* g1, const uint32_t* g2, size_t n, uint32_t* f) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   Aff<Fq> P; load_words_rw(P.x, g1 + i * 2 * Fq::WORDS); load_words_rw(P.y, g1 + i * 2 * Fq::WORDS + Fq::WORDS);
@@ -141,7 +146,7 @@ __global__ void __launch_bounds__(PAIR_THREADS) k_bls_miller(const uint32_t* g1,
 }
 
 // One level of the tree product: out[i] = in[2i] * in[2i + 1] (in[2i] alone when 2i + 1 = n). out may not alias in.
-__global__ void __launch_bounds__(PAIR_THREADS) k_bls_fold(const uint32_t* in, size_t n, uint32_t* out) {
+static __global__ void __launch_bounds__(PAIR_THREADS) k_bls_fold(const uint32_t* in, size_t n, uint32_t* out) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (2 * i >= n) return;
   Fq12 a = load_fq12(in + 2 * i * GT_WORDS);
@@ -150,7 +155,7 @@ __global__ void __launch_bounds__(PAIR_THREADS) k_bls_fold(const uint32_t* in, s
 }
 
 // One thread: gt = final_exponentiation(f), flag = (gt == 1)
-__global__ void __launch_bounds__(32) k_bls_final_exp(const uint32_t* f, uint32_t* gt, int* flag) {
+static __global__ void __launch_bounds__(32) k_bls_final_exp(const uint32_t* f, uint32_t* gt, int* flag) {
   if (threadIdx.x != 0) return;
   const Fq12 r = final_exponentiation(load_fq12(f));
   store_fq12(gt, r);

@@ -163,4 +163,35 @@ B200_DEV Fp12T<T> load_fq12(const uint32_t* src) {
   return f;
 }
 
+// ---- the per-call products of a batch of pairing checks (evm_bn254_pairing.cu, evm_bls12381_precompiles.cu) ----------------------
+// f holds one Miller value per pair, the pairs of a call contiguous: call c owns the values begin[c] .. begin[c + 1] - 1 (at least
+// one) and call_of[i] is the call of value i. FE::apply is the curve's final exponentiation.
+constexpr int PAIRING_THREADS = 64;
+
+// One level of the products of the calls, in place: at level `stride` = 2^l the value at offset j of its call, j a multiple of
+// 2 stride, takes the product with the value at j + stride when that exists; after ceil(log2(longest call)) levels each call's
+// product sits at offset 0.
+template <class T>
+__global__ void __launch_bounds__(PAIRING_THREADS) k_pairing_fold(uint32_t* f, const size_t* call_of, const size_t* begin, size_t n,
+                                                                  size_t stride) {
+  constexpr int GT_WORDS = 6 * T::Fq2::WORDS;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const size_t c = call_of[i], j = i - begin[c];
+  if (j % (2 * stride) != 0 || j + stride >= begin[c + 1] - begin[c]) return;
+  store_fq12(f + i * GT_WORDS, fq12_mul(load_fq12<T>(f + i * GT_WORDS), load_fq12<T>(f + (i + stride) * GT_WORDS)));
+}
+
+// One thread per call: ok[c] = (FE::apply(f[begin[c]]) == 1); gt (if not null) receives the GT values, ncalls x 12 Fp2 words
+template <class T, class FE>
+__global__ void __launch_bounds__(PAIRING_THREADS) k_pairing_final_exp(const uint32_t* f, const size_t* begin, size_t ncalls,
+                                                                       uint8_t* ok, uint32_t* gt) {
+  constexpr int GT_WORDS = 6 * T::Fq2::WORDS;
+  const size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= ncalls) return;
+  const Fp12T<T> r = FE::apply(load_fq12<T>(f + begin[c] * GT_WORDS));
+  ok[c] = r.is_one() ? 1 : 0;
+  if (gt) store_fq12(gt + c * GT_WORDS, r);
+}
+
 }  // namespace b200

@@ -445,6 +445,88 @@ def eth_evm_bn254_last_timing() -> dict:
     return dict(zip(("ms_host", "ms_decode", "ms_miller", "ms_final"), (x.value for x in v)))
 
 
+def eth_evm_bls12381_pairingcheck(inputs: bytes, out_len: int = 32):
+    """EIP-2537 BLS12_PAIRING_CHECK through ctt_eth_evm_bls12381_pairingcheck (reference constantine/ethereum_evm_precompiles.nim:
+    1064-1125): k x 384 bytes of (P.x, P.y, Q.x.c0, Q.x.c1, Q.y.c0, Q.y.c1), 64-byte big-endian each. Returns (status name, output
+    bytes), the output 32 bytes holding 0 or 1 (zeros when the call fails). The empty call is cttEVM_InvalidInputSize."""
+    r = ctypes.create_string_buffer(max(out_len, 1))
+    inputs = bytes(inputs)
+    st = _lib.load().ctt_eth_evm_bls12381_pairingcheck(r, out_len, inputs, len(inputs))
+    return EVM_STATUS[st], r.raw[:out_len]
+
+
+def eth_evm_bls12381_pairingcheck_batch(calls) -> list:
+    """Many independent BLS12_PAIRING_CHECK calls in one pass (ctt_b200_eth_evm_bls12381_pairingcheck_batch): calls is a sequence of
+    byte strings; returns [(status name, 32 output bytes)] in the same order, as the single entry gives them per call."""
+    calls = [bytes(c) for c in calls]
+    k = len(calls)
+    if k == 0:
+        return []
+    offsets = (ctypes.c_size_t * (k + 1))()
+    for i, c in enumerate(calls):
+        offsets[i + 1] = offsets[i] + len(c)
+    data = b"".join(calls) or b"\0"
+    r = ctypes.create_string_buffer(32 * k)
+    statuses = ctypes.create_string_buffer(k)
+    st = _lib.load().ctt_b200_eth_evm_bls12381_pairingcheck_batch(r, statuses, data, offsets[k], offsets, k)
+    if st != 0:
+        raise ValueError(EVM_STATUS[st])
+    raw = r.raw
+    return [(EVM_STATUS[statuses.raw[i]], raw[32 * i:32 * i + 32]) for i in range(k)]
+
+
+def _eth_evm_bls12381_map(name, inputs, out_len):
+    r = ctypes.create_string_buffer(max(out_len, 1))
+    inputs = bytes(inputs)
+    st = getattr(_lib.load(), name)(r, out_len, inputs, len(inputs))
+    return EVM_STATUS[st], r.raw[:out_len]
+
+
+def eth_evm_bls12381_map_fp_to_g1(inputs: bytes, out_len: int = 128):
+    """EIP-2537 BLS12_MAP_FP_TO_G1 through ctt_eth_evm_bls12381_map_fp_to_g1: u (64 bytes) -> (status name, the affine G1 point,
+    128 bytes; zeros for infinity)."""
+    return _eth_evm_bls12381_map("ctt_eth_evm_bls12381_map_fp_to_g1", inputs, out_len)
+
+
+def eth_evm_bls12381_map_fp2_to_g2(inputs: bytes, out_len: int = 256):
+    """EIP-2537 BLS12_MAP_FP2_TO_G2 through ctt_eth_evm_bls12381_map_fp2_to_g2: u = (c0, c1) (128 bytes) -> (status name, the affine
+    G2 point, 256 bytes; zeros for infinity)."""
+    return _eth_evm_bls12381_map("ctt_eth_evm_bls12381_map_fp2_to_g2", inputs, out_len)
+
+
+def _eth_evm_bls12381_map_batch(name, data, in_bytes):
+    data = bytes(data)
+    if len(data) % in_bytes:
+        raise ValueError("inputs must be a multiple of %d bytes" % in_bytes)
+    n = len(data) // in_bytes
+    r = ctypes.create_string_buffer(max(2 * in_bytes * n, 1))
+    statuses = ctypes.create_string_buffer(max(n, 1))
+    st = getattr(_lib.load(), name)(r, statuses, data or b"\0", n)
+    if st != 0:
+        raise ValueError(EVM_STATUS[st])
+    return [EVM_STATUS[b] for b in statuses.raw[:n]], r.raw[:2 * in_bytes * n]
+
+
+def eth_evm_bls12381_map_fp_to_g1_batch(data: bytes):
+    """n maps to G1 in one pass (ctt_b200_eth_evm_bls12381_map_fp_to_g1_batch): data is n x 64 bytes; returns ([status name] * n,
+    n x 128 output bytes), a failed element's output zeros."""
+    return _eth_evm_bls12381_map_batch("ctt_b200_eth_evm_bls12381_map_fp_to_g1_batch", data, 64)
+
+
+def eth_evm_bls12381_map_fp2_to_g2_batch(data: bytes):
+    """n maps to G2 in one pass (ctt_b200_eth_evm_bls12381_map_fp2_to_g2_batch): data is n x 128 bytes; returns ([status name] * n,
+    n x 256 output bytes), a failed element's output zeros."""
+    return _eth_evm_bls12381_map_batch("ctt_b200_eth_evm_bls12381_map_fp2_to_g2_batch", data, 128)
+
+
+def eth_evm_bls12381_last_timing() -> dict:
+    """Host checks and packing, device pair decoding, maps, Miller loops, and products with final exponentiations (ms) of the calling
+    thread's last EIP-2537 pairing-check or map call; phases the call does not have read 0."""
+    v = [ctypes.c_float(0) for _ in range(5)]
+    _lib.load().ctt_b200_eth_evm_bls12381_last_timing(*[ctypes.byref(x) for x in v])
+    return dict(zip(("ms_host", "ms_decode", "ms_map", "ms_miller", "ms_final"), (x.value for x in v)))
+
+
 class CtSpan(ctypes.Structure):
     """ctt_span: {byte* data; size_t len} (reference include/constantine/protocols/ethereum_bls_signatures.h:64)."""
     _fields_ = [("data", ctypes.c_void_p), ("len", ctypes.c_size_t)]

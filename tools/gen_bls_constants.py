@@ -7,6 +7,11 @@ Nothing here is copied from a table: every constant is computed from the curve.
     j = 0, and an isomorphism (x, y) -> (c^2 x, c^3 y) with c^6 = 4(1 + i) / B'' maps it onto E2: y^2 = x^3 + 4(1 + i). Of the
     finitely many (kernel, c) pairs, exactly one sends SSWU(u) to the RFC's Q0 and Q1 for every vector of tests/golden/bls_kat.json;
     the generator asserts that and keeps it.
+  - The 11-isogeny E1' -> E1 of the G1 SSWU map (RFC 9380, section 8.8.1), E1': y^2 = x^3 + A' x + B' with the RFC's A', B' and
+    Z = 11 (the generator asserts the RFC's conditions on Z): the kernel polynomial is the gcd of the 11-division polynomial of E1'
+    with x^p - x (degree 5, five Fp-rational roots: one kernel); Velu's formulas give a codomain with A'' = 0, and
+    (x, y) -> (c^2 x, c^3 y) with c^6 = 4 / B'' maps it onto E1: y^2 = x^3 + 4. Of the six c, exactly one sends SSWU(u0), SSWU(u1)
+    to Q0, Q1 for every RFC hash-to-G1 vector of tests/golden/eip2537_pairing_map_kat.json; the generator asserts that and keeps it.
   - psi(x, y) = (conj(x) cx, conj(y) cy) with cx = (1 + i)^(-(p - 1) / 3), cy = (1 + i)^(-(p - 1) / 2) (the untwist-Frobenius-twist
     endomorphism of the cofactor clearing, Budroni-Pintore).
   - The Frobenius of Fp12 = Fp2[w] / (w^6 - (1 + i)): w^k -> gamma_k w^k with gamma_k = (1 + i)^(k (p - 1) / 6), k = 1..5.
@@ -24,6 +29,7 @@ P = 0x1a0111ea397fe69a4b1ba7b6434bacd764774b84f38512bf6730d2a0f6b0f6241eabfffeb1
 R = 0x73eda753299d7d483339d80809a1d80553bda402fffe5bfeffffffff00000001
 X_ABS = 0xd201000000010000                     # the curve parameter is x = -X_ABS
 FIXTURE = os.path.join(ROOT, "tests", "golden", "bls_kat.json")
+FIXTURE_G1 = os.path.join(ROOT, "tests", "golden", "eip2537_pairing_map_kat.json")
 OUT = os.path.join(ROOT, "constantine_b200", "csrc", "bls_constants.cuh")
 OUT_CODEC = os.path.join(ROOT, "constantine_b200", "csrc", "codec_constants.cuh")
 G1_GEN = (0x17f1d3a73197d7942695638c4fa9ac0fc3688c4f9774b905a14e3a3f171bac586c55e83ff97a1aeffb3af00adb22c6bb,
@@ -354,6 +360,228 @@ def load_rfc_vectors():
         return json.load(f)["rfc_h2c"]["vectors"]
 
 
+# ---- the G1 map: simplified SWU on E1' and the 11-isogeny E1' -> E1 (RFC 9380 section 8.8.1) -----------------------------------
+A1_ISO = 0x144698a3b8e9433d693a02c96d4982b0ea985383ee66a8d8e8981aefd881ac98936f8da0e0f97f5cf428082d584c1d   # E1': y^2 = x^3 + A' x + B'
+B1_ISO = 0x12e2908d11688030018b12e8753eee3b2016c1f0f24f4070a0b9c14fcef35ef55a23215a316ceaa5d1cc48e98e172be0
+Z1_SSWU = 11
+B_E1 = 4                                        # E1: y^2 = x^3 + 4
+
+
+def fp_is_square(a):
+    return a % P == 0 or pow(a, (P - 1) // 2, P) == 1
+
+
+def fp_sqrt(a):
+    """A square root of a in Fp (p = 3 mod 4), or None."""
+    y = pow(a, (P + 1) // 4, P)
+    return y if y * y % P == a % P else None
+
+
+def check_z1():
+    """RFC 9380 section 6.6.2 (and H.2): Z is a non-square, Z != -1, x^2 + A' x + B' - Z is irreducible (no root in Fp), and
+    g(B' / (Z A')) is a square."""
+    A, B, Z = A1_ISO, B1_ISO, Z1_SSWU
+    assert not fp_is_square(Z) and Z != P - 1
+    assert not fp_is_square((A * A - 4 * (B - Z)) % P)    # the discriminant of x^2 + A x + (B - Z) is a non-square
+    x = B * pow(Z * A, -1, P) % P
+    assert fp_is_square((x ** 3 + A * x + B) % P)
+
+
+def sswu_g1(u):
+    """simplified SWU on E1' (the plain non-constant-time form), sgn0 = the parity of the canonical value (m = 1)"""
+    A, B, Z = A1_ISO, B1_ISO, Z1_SSWU
+    zu2 = Z * u * u % P
+    den = (zu2 * zu2 + zu2) % P
+    if den == 0:
+        x1 = B * pow(Z * A, -1, P) % P
+    else:
+        x1 = -B * pow(A, -1, P) * (1 + pow(den, -1, P)) % P
+    gx1 = (x1 ** 3 + A * x1 + B) % P
+    if fp_is_square(gx1):
+        x, y = x1, fp_sqrt(gx1)
+    else:
+        x = zu2 * x1 % P
+        y = fp_sqrt((x ** 3 + A * x + B) % P)
+    if (u & 1) != (y & 1):
+        y = (-y) % P
+    return x, y
+
+
+# polynomials over Fp: coefficient lists of ints, lowest degree first
+def q_trim(f):
+    while f and f[-1] == 0:
+        f = f[:-1]
+    return f
+
+
+def q_add(f, g):
+    n = max(len(f), len(g))
+    return q_trim([((f[i] if i < len(f) else 0) + (g[i] if i < len(g) else 0)) % P for i in range(n)])
+
+
+def q_scale(k, f):
+    return q_trim([k * a % P for a in f])
+
+
+def q_mul(f, g):
+    if not f or not g:
+        return []
+    r = [0] * (len(f) + len(g) - 1)
+    for i, a in enumerate(f):
+        for j, b in enumerate(g):
+            r[i + j] += a * b
+    return q_trim([c % P for c in r])
+
+
+def q_divmod(f, g):
+    f = list(f)
+    ig = pow(g[-1], -1, P)
+    qt = [0] * max(0, len(f) - len(g) + 1)
+    while len(f) >= len(g):
+        c = f[-1] * ig % P
+        s = len(f) - len(g)
+        qt[s] = c
+        for i in range(len(g)):
+            f[s + i] = (f[s + i] - c * g[i]) % P
+        f = q_trim(f[:-1])
+    return q_trim(qt), q_trim(f)
+
+
+def q_powmod(base, e, m):
+    r, b = [1], q_divmod(base, m)[1]
+    while e:
+        if e & 1:
+            r = q_divmod(q_mul(r, b), m)[1]
+        b = q_divmod(q_mul(b, b), m)[1]
+        e >>= 1
+    return r
+
+
+def q_gcd(f, g):
+    f, g = q_trim(f), q_trim(g)
+    while g:
+        f, g = g, q_divmod(f, g)[1]
+    return q_scale(pow(f[-1], -1, P), f)
+
+
+def q_eval(f, x):
+    r = 0
+    for c in reversed(f):
+        r = (r * x + c) % P
+    return r
+
+
+def q_roots(f, rng):
+    """The roots in Fp of a squarefree product of distinct linear factors f (equal-degree splitting)."""
+    if len(f) <= 1:
+        return []
+    if len(f) == 2:
+        return [(-f[0]) * pow(f[1], -1, P) % P]
+    while True:
+        h = q_add(q_powmod([rng.randrange(P), 1], (P - 1) // 2, f), [P - 1])
+        k = q_gcd(f, h) if h else f
+        if 1 < len(k) < len(f):
+            return q_roots(k, rng) + q_roots(q_divmod(f, k)[0], rng)
+
+
+def division_polynomial_11():
+    """psi_11 of E1' as a polynomial in x (odd n: psi_n is a polynomial; even n: psi_n = y h_n(x), with y^2 = x^3 + A' x + B')"""
+    A, B = A1_ISO, B1_ISO
+    F = [B, A, 0, 1]
+    F2 = q_mul(F, F)
+    h = {0: [], 1: [1], 2: [2],
+         3: q_trim([(-A * A) % P, 12 * B % P, 6 * A % P, 0, 3]),
+         4: q_scale(4, [(-8 * B * B - A ** 3) % P, (-4 * A * B) % P, (-5 * A * A) % P, 20 * B % P, 5 * A % P, 0, 1])}
+    inv2 = pow(2, -1, P)
+    for n in range(5, 12):
+        m = n // 2
+        if n % 2:        # psi_{2m+1} = psi_{m+2} psi_m^3 - psi_{m-1} psi_{m+1}^3; the even factors carry y^4 = F^2
+            a = q_mul(h[m + 2], q_mul(h[m], q_mul(h[m], h[m])))
+            b = q_mul(h[m - 1], q_mul(h[m + 1], q_mul(h[m + 1], h[m + 1])))
+            if m % 2 == 0:
+                a = q_mul(a, F2)
+            else:
+                b = q_mul(b, F2)
+            h[n] = q_add(a, q_scale(P - 1, b))
+        else:            # psi_{2m} = (psi_{m+2} psi_{m-1}^2 - psi_{m-2} psi_{m+1}^2) psi_m / (2y)
+            t = q_add(q_mul(h[m + 2], q_mul(h[m - 1], h[m - 1])), q_scale(P - 1, q_mul(h[m - 2], q_mul(h[m + 1], h[m + 1]))))
+            h[n] = q_scale(inv2, q_mul(t, h[m]))
+    assert len(h[11]) == 61 and h[11][-1] == 11
+    return h[11]
+
+
+def g1_iso_candidates():
+    """The kernel of the Fp-rational 11-isogeny (the Fp-rational roots of psi_11: its gcd with x^p - x), the codomain by Velu's
+    formulas (A'' = 0 for this kernel), and every c with c^6 = 4 / B''. Returns (the kernel's x-coordinates, [c, ...])."""
+    rng = random.Random(1381)
+    A, B = A1_ISO, B1_ISO
+    psi11 = division_polynomial_11()
+    kernel = q_gcd(psi11, q_add(q_powmod([0, 1], P, psi11), [0, P - 1]))
+    assert len(kernel) == 6, "expected one Fp-rational 11-isogeny kernel (a gcd of degree 5), got degree %d" % (len(kernel) - 1)
+    xs = q_roots(kernel, rng)
+    assert len(xs) == 5
+    t = sum(2 * (3 * x * x + A) for x in xs) % P                 # Velu: t_Q = 6 x_Q^2 + 2A, u_Q = 4 y_Q^2
+    w = sum(4 * (x ** 3 + A * x + B) + x * 2 * (3 * x * x + A) for x in xs) % P
+    a2, b2 = (A - 5 * t) % P, (B - 7 * w) % P
+    assert a2 == 0, "the 11-isogenous curve has j != 0"
+    c6 = B_E1 * pow(b2, -1, P) % P
+    cs = q_roots(q_gcd([(-c6) % P, 0, 0, 0, 0, 0, 1], q_add(q_powmod([0, 1], P, [(-c6) % P, 0, 0, 0, 0, 0, 1]), [0, P - 1])), rng)
+    assert len(cs) == 6, "4 / B'' is not a sixth power in Fp"
+    return xs, cs
+
+
+def g1_iso_polys(xs, c):
+    """Velu's isogeny with the kernel over xs, composed with (x, y) -> (c^2 x, c^3 y): x -> x_num / x_den, y -> y y_num / y_den;
+    x_den = D^2, y_den = D^3 with D = prod (x - x_Q) (monic), x_num of degree 11, y_num of degree 15.
+      X = x + sum_Q (t_Q (x - x_Q) + u_Q) / (x - x_Q)^2,   Y = y (1 - sum_Q (t_Q (x - x_Q) + 2 u_Q) / (x - x_Q)^3)"""
+    A, B = A1_ISO, B1_ISO
+    D = [1]
+    for x0 in xs:
+        D = q_mul(D, [(-x0) % P, 1])
+    D2, D3 = q_mul(D, D), q_mul(q_mul(D, D), D)
+    xn, yn = q_mul([0, 1], D2), D3
+    for x0 in xs:
+        tq, uq = 2 * (3 * x0 * x0 + A) % P, 4 * (x0 ** 3 + A * x0 + B) % P
+        lin = [(-x0) % P, 1]
+        rest2 = q_divmod(D2, q_mul(lin, lin))[0]
+        rest3 = q_divmod(D3, q_mul(lin, q_mul(lin, lin)))[0]
+        xn = q_add(xn, q_mul(q_add(q_scale(tq, lin), [uq]), rest2))
+        yn = q_add(yn, q_scale(P - 1, q_mul(q_add(q_scale(tq, lin), [2 * uq % P]), rest3)))
+    c2, c3 = c * c % P, c * c * c % P
+    return q_scale(c2, xn), D2, q_scale(c3, yn), D3
+
+
+def g1_iso_apply(polys, pt):
+    """the isogeny at an affine point of E1'; None (the identity) where a denominator vanishes"""
+    xn, xd, yn, yd = polys
+    x, y = pt
+    dx, dy = q_eval(xd, x), q_eval(yd, x)
+    if dx == 0 or dy == 0:
+        return None
+    return q_eval(xn, x) * pow(dx, -1, P) % P, y * q_eval(yn, x) * pow(dy, -1, P) % P
+
+
+def select_g1_isogeny(vectors):
+    """The unique c that maps SSWU(u0), SSWU(u1) to the RFC's Q0, Q1 for every G1 vector."""
+    check_z1()
+    xs, cs = g1_iso_candidates()
+    good = []
+    for c in cs:
+        polys = g1_iso_polys(xs, c)
+        if all(g1_iso_apply(polys, sswu_g1(int(v[uk], 16))) == (int(v[qk]["x"], 16), int(v[qk]["y"], 16))
+               for v in vectors for uk, qk in (("u0", "Q0"), ("u1", "Q1"))):
+            good.append(polys)
+    assert len(good) == 1, "expected exactly one G1 isogeny candidate to match the RFC vectors, found %d" % len(good)
+    xn, xd, yn, yd = good[0]
+    assert (len(xn), len(xd), len(yn), len(yd)) == (12, 11, 16, 16)
+    return good[0]
+
+
+def load_rfc_g1_vectors():
+    with open(FIXTURE_G1) as f:
+        return json.load(f)["rfc_h2g1"]["vectors"]
+
+
 # ---- header ------------------------------------------------------------------------------------------------------------------
 def mont_words(a):
     m = (a * (1 << 384)) % P
@@ -364,8 +592,8 @@ def fp2_words(a):
     return mont_words(a[0]) + mont_words(a[1])
 
 
-def emit(name, elems):
-    words = [w for e in elems for w in fp2_words(e)]
+def emit(name, elems, words_of=fp2_words):
+    words = [w for e in elems for w in words_of(e)]
     lines = ["__device__ __constant__ uint32_t %s[%d] = {" % (name, len(words))]
     for k in range(0, len(words), 8):
         lines.append("    " + ", ".join("0x%08xu" % w for w in words[k:k + 8]) + ",")
@@ -375,6 +603,7 @@ def emit(name, elems):
 
 def header_text():
     xn, xd, yn, yd = select_isogeny(load_rfc_vectors())
+    g1n, g1d, g1yn, g1yd = select_g1_isogeny(load_rfc_g1_vectors())
     cx, cy = psi_constants()
     body = [
         "// GENERATED by tools/gen_bls_constants.py -- derived from the curve, see that file. Fp2 elements as 24 little-endian 32-bit",
@@ -391,6 +620,11 @@ def header_text():
         emit("H2C_ISO", xn + xd + yn + yd),
         "// psi(x, y) = (conj(x) cx, conj(y) cy)",
         emit("H2C_PSI", [cx, cy]),
+        "// SSWU on E1' (Fp elements, 12 words each): A', B', Z = 11",
+        emit("H2C_G1_SSWU", [A1_ISO, B1_ISO, Z1_SSWU], mont_words),
+        "// the 11-isogeny E1' -> E1: x = x_num(x') / x_den(x'), y = y' y_num(x') / y_den(x'); coefficients lowest degree first,",
+        "// x_num (12), x_den (11, monic), y_num (16), y_den (16, monic)",
+        emit("H2C_G1_ISO", g1n + g1d + g1yn + g1yd, mont_words),
         "// Frobenius of Fp12: gamma_k = (1 + i)^(k (p - 1) / 6), k = 1..5",
         emit("PAIR_FROB", frobenius_constants()),
         "}  // namespace bls",
@@ -429,7 +663,7 @@ def write_if_changed(path, text):
 def main():
     write_if_changed(OUT, header_text())
     write_if_changed(OUT_CODEC, codec_header_text())
-    print("bls constants: one isogeny of %d candidates matches the RFC vectors" % len(iso_candidates()))
+    print("bls constants: one G2 isogeny of %d candidates and one G1 isogeny of 6 match the RFC vectors" % len(iso_candidates()))
 
 
 if __name__ == "__main__":
