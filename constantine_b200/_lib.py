@@ -114,6 +114,15 @@ def load():
         fn.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_evm_bls12381_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 5
     lib.ctt_b200_eth_evm_bls12381_last_timing.restype = None
+    for nm in ("bn254_g1add", "bn254_g1mul", "bls12381_g1add", "bls12381_g2add", "bls12381_g1mul", "bls12381_g2mul"):
+        fn = getattr(lib, "ctt_eth_evm_" + nm)
+        fn.argtypes = [vp, sz, vp, sz]
+        fn.restype = ctypes.c_ubyte
+        fn = getattr(lib, "ctt_b200_eth_evm_" + nm + "_batch")
+        fn.argtypes = [vp, vp, vp, sz]
+        fn.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_evm_ecops_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)]
+    lib.ctt_b200_eth_evm_ecops_last_timing.restype = None
     lib.ctt_b200_test_bn254_pairing.argtypes = [vp, vp, sz, vp]
     lib.ctt_b200_test_bn254_pairing.restype = ci
     lib.ctt_b200_eth_kzg_context_new.argtypes = [vp]

@@ -166,6 +166,17 @@ B200_DEV void load_be32(const uint8_t* s, uint32_t* w) {
     w[4 - 4 * k] = __byte_perm(v.w, 0, 0x0123);
   }
 }
+// a Montgomery element -> 32 canonical big-endian bytes (16-byte aligned)
+B200_DEV void store_be32(uint8_t* d, const Fq& a) {
+  Fq one_raw = Fq::zero();
+  one_raw.l[0] = 1;
+  const Fq c = a * one_raw;
+  uint4* q = reinterpret_cast<uint4*>(d);
+#pragma unroll
+  for (int k = 0; k < 2; k++)
+    q[k] = make_uint4(__byte_perm(c.l[7 - 4 * k], 0, 0x0123), __byte_perm(c.l[6 - 4 * k], 0, 0x0123),
+                      __byte_perm(c.l[5 - 4 * k], 0, 0x0123), __byte_perm(c.l[4 - 4 * k], 0, 0x0123));
+}
 B200_DEV bool geq_p(const uint32_t* w) {
 #pragma unroll 1
   for (int i = 7; i >= 0; i--)

@@ -13,6 +13,13 @@
 // Per batch, on one engine lease and stream: pairing checks run the decoder (statuses, curve and subgroup checks), one Miller loop
 // per pair (k_bls_miller), the levels of each call's product and one final exponentiation per call (tower.cuh); maps run one kernel
 // that writes the wire output and the statuses. There is no CPU path.
+//
+// EIP-2537 BLS12_G1ADD, G2ADD, G1MUL and G2MUL: ctt_eth_evm_bls12381_g{1,2}{add,mul} (the reference's names and prototypes; Nim
+// source constantine/ethereum_evm_precompiles.nim:628-892), and batch entries of many independent calls. The input length (256 /
+// 512 / 160 / 288) is checked before the output length (128 / 256), then P and Q (additions) or P (multiplications) in order: every
+// coordinate in range, then all zeros is infinity, else on the curve (twist), and for the multiplications in G1 (G2). The additions
+// do not check the subgroup. The scalar is any 256-bit value, reduced mod r. Per batch one engine lease and stream, one kernel
+// (ecops_kernels.cuh) that writes the wire output and the statuses.
 #define CTT_B200_BUILDING_LIBRARY
 #include "../../include/ctt_b200_msm.h"
 #include "msm_hooks.cuh"
@@ -175,6 +182,65 @@ static uint8_t map_one(bool g2, uint8_t* r, size_t r_len, const uint8_t* inputs,
   return status;
 }
 
+// BLS12_G1ADD / G1MUL and BLS12_G2ADD / G2MUL (ecops_kernels.cuh): E y^2 = x^3 + 4 and the twist y^2 = x^3 + 4(1 + i)
+struct G1Wire {
+  using F = Fq;
+  using Fr = Bls12381Fr;
+  static constexpr int FBYTES = 64, R_SUBS = 2;
+  static constexpr bool SUBGROUP = true;
+  static B200_DEV bool load(const uint8_t* s, F& a) {
+    uint32_t w[12];
+    if (!load_coord(s, w)) return false;
+    a = codec::to_mont(w);
+    return true;
+  }
+  static B200_DEV void store(uint8_t* d, const F& a) { store_coord(d, a); }
+  static B200_DEV F b() { return F::one().dbl().dbl(); }
+  static __device__ bool in_subgroup(const Aff<F>& p) { return codec::g1_in_subgroup(p.x, p.y); }
+};
+struct G2Wire {
+  using F = Fq2;
+  using Fr = Bls12381Fr;
+  static constexpr int FBYTES = 128, R_SUBS = 2;
+  static constexpr bool SUBGROUP = true;
+  static B200_DEV bool load(const uint8_t* s, F& a) { return G1Wire::load(s, a.c0) && G1Wire::load(s + 64, a.c1); }
+  static B200_DEV void store(uint8_t* d, const F& a) { store_coord(d, a.c0); store_coord(d + 64, a.c1); }
+  static B200_DEV F b() { F b; b.c0 = G1Wire::b(); b.c1 = b.c0; return b; }
+  static __device__ bool in_subgroup(const Aff<F>& p) { return codec::g2_in_subgroup(p.x, p.y); }
+};
+
+enum EcOp { G1ADD, G2ADD, G1MUL, G2MUL };
+constexpr size_t ECOP_IN[] = {256, 512, 160, 288}, ECOP_OUT[] = {128, 256, 128, 256};
+
+// n records of ECOP_IN[op] bytes -> n x ECOP_OUT[op] bytes and n statuses
+static uint8_t ecop_batch(EcOp op, uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t n) {
+  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return EVM_INVALID_INPUT_SIZE;
+  ecops::last_ms() = 0;
+  if (n == 0) return EVM_SUCCESS;
+  EngineLease lease = acquire_engine();
+  cudaStream_t s = lease.e->compute();
+  float ms = 0;
+  switch (op) {
+    case G1ADD: ms = ecops::run_batch<G1Wire, false>(s, r, statuses, inputs, n); break;
+    case G2ADD: ms = ecops::run_batch<G2Wire, false>(s, r, statuses, inputs, n); break;
+    case G1MUL: ms = ecops::run_batch<G1Wire, true>(s, r, statuses, inputs, n); break;
+    case G2MUL: ms = ecops::run_batch<G2Wire, true>(s, r, statuses, inputs, n); break;
+  }
+  ecops::last_ms() = ms;
+  return EVM_SUCCESS;
+}
+
+// the single entries: input size, then output size, then the batch of one; r is written only on success
+static uint8_t ecop_one(EcOp op, uint8_t* r, size_t r_len, const uint8_t* inputs, size_t inputs_len) {
+  ecops::last_ms() = 0;
+  if (inputs_len != ECOP_IN[op] || !inputs) return EVM_INVALID_INPUT_SIZE;
+  if (r_len != ECOP_OUT[op] || !r) return EVM_INVALID_OUTPUT_SIZE;
+  uint8_t out[256], status;
+  ecop_batch(op, out, &status, inputs, 1);
+  if (status == EVM_SUCCESS) memcpy(r, out, ECOP_OUT[op]);
+  return status;
+}
+
 }  // namespace evmbls
 }  // namespace b200
 
@@ -215,6 +281,42 @@ ctt_evm_status ctt_b200_eth_evm_bls12381_map_fp_to_g1_batch(byte* r, byte* statu
 
 ctt_evm_status ctt_b200_eth_evm_bls12381_map_fp2_to_g2_batch(byte* r, byte* statuses, const byte* inputs, size_t n) {
   return (ctt_evm_status)evmbls::map_batch(true, r, statuses, inputs, n);
+}
+
+// reference include/constantine/protocols/ethereum_evm_precompiles.h (eth_evm_bls12381_g1add)
+ctt_evm_status ctt_eth_evm_bls12381_g1add(byte* r, size_t r_len, const byte* inputs, size_t inputs_len) {
+  return (ctt_evm_status)evmbls::ecop_one(evmbls::G1ADD, r, r_len, inputs, inputs_len);
+}
+
+// reference include/constantine/protocols/ethereum_evm_precompiles.h (eth_evm_bls12381_g2add)
+ctt_evm_status ctt_eth_evm_bls12381_g2add(byte* r, size_t r_len, const byte* inputs, size_t inputs_len) {
+  return (ctt_evm_status)evmbls::ecop_one(evmbls::G2ADD, r, r_len, inputs, inputs_len);
+}
+
+// reference include/constantine/protocols/ethereum_evm_precompiles.h (eth_evm_bls12381_g1mul)
+ctt_evm_status ctt_eth_evm_bls12381_g1mul(byte* r, size_t r_len, const byte* inputs, size_t inputs_len) {
+  return (ctt_evm_status)evmbls::ecop_one(evmbls::G1MUL, r, r_len, inputs, inputs_len);
+}
+
+// reference include/constantine/protocols/ethereum_evm_precompiles.h (eth_evm_bls12381_g2mul)
+ctt_evm_status ctt_eth_evm_bls12381_g2mul(byte* r, size_t r_len, const byte* inputs, size_t inputs_len) {
+  return (ctt_evm_status)evmbls::ecop_one(evmbls::G2MUL, r, r_len, inputs, inputs_len);
+}
+
+ctt_evm_status ctt_b200_eth_evm_bls12381_g1add_batch(byte* r, byte* statuses, const byte* inputs, size_t n) {
+  return (ctt_evm_status)evmbls::ecop_batch(evmbls::G1ADD, r, statuses, inputs, n);
+}
+
+ctt_evm_status ctt_b200_eth_evm_bls12381_g2add_batch(byte* r, byte* statuses, const byte* inputs, size_t n) {
+  return (ctt_evm_status)evmbls::ecop_batch(evmbls::G2ADD, r, statuses, inputs, n);
+}
+
+ctt_evm_status ctt_b200_eth_evm_bls12381_g1mul_batch(byte* r, byte* statuses, const byte* inputs, size_t n) {
+  return (ctt_evm_status)evmbls::ecop_batch(evmbls::G1MUL, r, statuses, inputs, n);
+}
+
+ctt_evm_status ctt_b200_eth_evm_bls12381_g2mul_batch(byte* r, byte* statuses, const byte* inputs, size_t n) {
+  return (ctt_evm_status)evmbls::ecop_batch(evmbls::G2MUL, r, statuses, inputs, n);
 }
 
 void ctt_b200_eth_evm_bls12381_last_timing(float* ms_host, float* ms_decode, float* ms_map, float* ms_miller, float* ms_final) {

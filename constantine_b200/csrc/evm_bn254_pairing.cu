@@ -12,10 +12,17 @@
 // Per batch: host, the call-level checks and the packing of the pairs of the calls that need a pairing; device (one engine lease and
 // stream), the decoder (statuses, curve and subgroup checks), one Miller loop per pair, the levels of each call's product, one final
 // exponentiation per call; the pair statuses and one flag per call come back. There is no CPU path.
+//
+// EIP-196 ECADD / ECMUL: ctt_eth_evm_bn254_g1add and ctt_eth_evm_bn254_g1mul (the reference's names and prototypes; Nim source
+// constantine/ethereum_evm_precompiles.nim:413-541), and batch entries of many independent calls. The output size is checked first
+// (64 bytes); the input is zero-padded or truncated to 128 (96) bytes, so there is no input-size error; then P and Q (ECADD) or P
+// (ECMUL) in order: coordinates < p, then (0, 0) is infinity, else on the curve. The scalar is any 256-bit value, reduced mod r.
+// Per batch one engine lease and stream, one kernel (ecops_kernels.cuh) that writes the wire output and the statuses.
 #define CTT_B200_BUILDING_LIBRARY
 #include "../../include/ctt_b200_msm.h"
 #include "msm_hooks.cuh"
 #include "bn254_pairing_kernels.cuh"
+#include "ecops_kernels.cuh"
 #include <algorithm>
 #include <chrono>
 #include <cstring>
@@ -104,6 +111,49 @@ static double ms_since(std::chrono::steady_clock::time_point t0) {
   return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
 
+// EIP-196 ECADD / ECMUL (ecops_kernels.cuh): G1 y^2 = x^3 + 3, 32-byte big-endian coordinates < p, (0, 0) infinity, cofactor 1
+struct G1Wire {
+  using F = bn::Fq;
+  using Fr = Bn254SnarksFr;
+  static constexpr int FBYTES = 32, R_SUBS = 5;
+  static constexpr bool SUBGROUP = false;
+  static B200_DEV bool load(const uint8_t* s, F& a) {
+    uint32_t w[8];
+    bn::load_be32(s, w);
+    if (bn::geq_p(w)) return false;
+    a = bn::to_mont(w);
+    return true;
+  }
+  static B200_DEV void store(uint8_t* d, const F& a) { bn::store_be32(d, a); }
+  static B200_DEV F b() { return F::one().dbl() + F::one(); }
+};
+constexpr size_t ADD_BYTES = 128, MUL_BYTES = 96, OUT_BYTES = 64;
+
+// n records of ADD_BYTES (MUL_BYTES) -> n x OUT_BYTES and n statuses
+static uint8_t ecop_batch(bool mul, uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t n) {
+  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return bn::EVM_INVALID_INPUT_SIZE;
+  ecops::last_ms() = 0;
+  if (n == 0) return bn::EVM_SUCCESS;
+  EngineLease lease = acquire_engine();
+  cudaStream_t s = lease.e->compute();
+  ecops::last_ms() = mul ? ecops::run_batch<G1Wire, true>(s, r, statuses, inputs, n)
+                         : ecops::run_batch<G1Wire, false>(s, r, statuses, inputs, n);
+  return bn::EVM_SUCCESS;
+}
+
+// the single entries: the output size, then the input zero-padded or truncated to one record; r is written only on success
+static uint8_t ecop_one(bool mul, uint8_t* r, size_t r_len, const uint8_t* inputs, size_t inputs_len) {
+  ecops::last_ms() = 0;
+  if (r_len != OUT_BYTES || !r) return bn::EVM_INVALID_OUTPUT_SIZE;
+  if (!inputs && inputs_len) return bn::EVM_INVALID_INPUT_SIZE;
+  const size_t in_bytes = mul ? MUL_BYTES : ADD_BYTES;
+  uint8_t in[ADD_BYTES] = {}, out[OUT_BYTES], status;
+  if (inputs_len) memcpy(in, inputs, std::min(inputs_len, in_bytes));
+  ecop_batch(mul, out, &status, in, 1);
+  if (status == bn::EVM_SUCCESS) memcpy(r, out, OUT_BYTES);
+  return status;
+}
+
 // k calls, call i = inputs[offsets[i], offsets[i + 1]); r: k x 32 bytes, statuses: k bytes
 static uint8_t pairing_check_batch(uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t inputs_len, const size_t* offsets,
                                    size_t k) {
@@ -177,6 +227,28 @@ void ctt_b200_eth_evm_bn254_last_timing(float* ms_host, float* ms_decode, float*
   if (ms_decode) *ms_decode = t.ms_decode;
   if (ms_miller) *ms_miller = t.ms_miller;
   if (ms_final) *ms_final = t.ms_final;
+}
+
+// reference include/constantine/protocols/ethereum_evm_precompiles.h (eth_evm_bn254_g1add)
+ctt_evm_status ctt_eth_evm_bn254_g1add(byte* r, size_t r_len, const byte* inputs, size_t inputs_len) {
+  return (ctt_evm_status)evmbn::ecop_one(false, r, r_len, inputs, inputs_len);
+}
+
+// reference include/constantine/protocols/ethereum_evm_precompiles.h (eth_evm_bn254_g1mul)
+ctt_evm_status ctt_eth_evm_bn254_g1mul(byte* r, size_t r_len, const byte* inputs, size_t inputs_len) {
+  return (ctt_evm_status)evmbn::ecop_one(true, r, r_len, inputs, inputs_len);
+}
+
+ctt_evm_status ctt_b200_eth_evm_bn254_g1add_batch(byte* r, byte* statuses, const byte* inputs, size_t n) {
+  return (ctt_evm_status)evmbn::ecop_batch(false, r, statuses, inputs, n);
+}
+
+ctt_evm_status ctt_b200_eth_evm_bn254_g1mul_batch(byte* r, byte* statuses, const byte* inputs, size_t n) {
+  return (ctt_evm_status)evmbn::ecop_batch(true, r, statuses, inputs, n);
+}
+
+void ctt_b200_eth_evm_ecops_last_timing(float* ms_kernel) {
+  if (ms_kernel) *ms_kernel = ecops::last_ms();
 }
 
 int ctt_b200_test_bn254_pairing(const void* g1_aff, const void* g2_aff, size_t n, void* gt_out) {

@@ -527,6 +527,105 @@ def eth_evm_bls12381_last_timing() -> dict:
     return dict(zip(("ms_host", "ms_decode", "ms_map", "ms_miller", "ms_final"), (x.value for x in v)))
 
 
+# EVM curve operations: name -> (record bytes of a batch, output bytes)
+ECOPS = {"bn254_g1add": (128, 64), "bn254_g1mul": (96, 64), "bls12381_g1add": (256, 128), "bls12381_g2add": (512, 256),
+         "bls12381_g1mul": (160, 128), "bls12381_g2mul": (288, 256)}
+
+
+def _eth_evm_ecop(name, inputs, out_len):
+    r = ctypes.create_string_buffer(max(out_len, 1))
+    inputs = bytes(inputs)
+    st = getattr(_lib.load(), "ctt_eth_evm_" + name)(r, out_len, inputs, len(inputs))
+    return EVM_STATUS[st], r.raw[:out_len]
+
+
+def eth_evm_bn254_g1add(inputs: bytes, out_len: int = 64):
+    """EIP-196 ECADD through ctt_eth_evm_bn254_g1add: P, Q (32-byte big-endian coordinates; the input zero-padded or truncated to
+    128 bytes) -> (status name, P + Q affine, 64 bytes; zeros for infinity)."""
+    return _eth_evm_ecop("bn254_g1add", inputs, out_len)
+
+
+def eth_evm_bn254_g1mul(inputs: bytes, out_len: int = 64):
+    """EIP-196 ECMUL through ctt_eth_evm_bn254_g1mul: P and a 32-byte scalar (padded or truncated to 96 bytes) -> (status name,
+    [s]P affine, 64 bytes)."""
+    return _eth_evm_ecop("bn254_g1mul", inputs, out_len)
+
+
+def eth_evm_bls12381_g1add(inputs: bytes, out_len: int = 128):
+    """EIP-2537 BLS12_G1ADD through ctt_eth_evm_bls12381_g1add: P, Q (256 bytes) -> (status name, P + Q, 128 bytes)."""
+    return _eth_evm_ecop("bls12381_g1add", inputs, out_len)
+
+
+def eth_evm_bls12381_g2add(inputs: bytes, out_len: int = 256):
+    """EIP-2537 BLS12_G2ADD through ctt_eth_evm_bls12381_g2add: P, Q (512 bytes) -> (status name, P + Q, 256 bytes)."""
+    return _eth_evm_ecop("bls12381_g2add", inputs, out_len)
+
+
+def eth_evm_bls12381_g1mul(inputs: bytes, out_len: int = 128):
+    """EIP-2537 BLS12_G1MUL through ctt_eth_evm_bls12381_g1mul: P and a 32-byte scalar (160 bytes) -> (status name, [s]P, 128
+    bytes); P must be in G1."""
+    return _eth_evm_ecop("bls12381_g1mul", inputs, out_len)
+
+
+def eth_evm_bls12381_g2mul(inputs: bytes, out_len: int = 256):
+    """EIP-2537 BLS12_G2MUL through ctt_eth_evm_bls12381_g2mul: P and a 32-byte scalar (288 bytes) -> (status name, [s]P, 256
+    bytes); P must be in G2."""
+    return _eth_evm_ecop("bls12381_g2mul", inputs, out_len)
+
+
+def _eth_evm_ecop_batch(name, data):
+    in_bytes, out_bytes = ECOPS[name]
+    data = bytes(data)
+    if len(data) % in_bytes:
+        raise ValueError("inputs must be a multiple of %d bytes" % in_bytes)
+    n = len(data) // in_bytes
+    r = ctypes.create_string_buffer(max(out_bytes * n, 1))
+    statuses = ctypes.create_string_buffer(max(n, 1))
+    st = getattr(_lib.load(), "ctt_b200_eth_evm_" + name + "_batch")(r, statuses, data or b"\0", n)
+    if st != 0:
+        raise ValueError(EVM_STATUS[st])
+    return [EVM_STATUS[b] for b in statuses.raw[:n]], r.raw[:out_bytes * n]
+
+
+def eth_evm_bn254_g1add_batch(data: bytes):
+    """n ECADD calls in one pass (ctt_b200_eth_evm_bn254_g1add_batch): data is n x 128 bytes; returns ([status name] * n, n x 64
+    output bytes), a failed record's output zeros."""
+    return _eth_evm_ecop_batch("bn254_g1add", data)
+
+
+def eth_evm_bn254_g1mul_batch(data: bytes):
+    """n ECMUL calls in one pass: data is n x 96 bytes; returns ([status name] * n, n x 64 output bytes)."""
+    return _eth_evm_ecop_batch("bn254_g1mul", data)
+
+
+def eth_evm_bls12381_g1add_batch(data: bytes):
+    """n BLS12_G1ADD calls in one pass: data is n x 256 bytes; returns ([status name] * n, n x 128 output bytes)."""
+    return _eth_evm_ecop_batch("bls12381_g1add", data)
+
+
+def eth_evm_bls12381_g2add_batch(data: bytes):
+    """n BLS12_G2ADD calls in one pass: data is n x 512 bytes; returns ([status name] * n, n x 256 output bytes)."""
+    return _eth_evm_ecop_batch("bls12381_g2add", data)
+
+
+def eth_evm_bls12381_g1mul_batch(data: bytes):
+    """n BLS12_G1MUL calls in one pass: data is n x 160 bytes; returns ([status name] * n, n x 128 output bytes)."""
+    return _eth_evm_ecop_batch("bls12381_g1mul", data)
+
+
+def eth_evm_bls12381_g2mul_batch(data: bytes):
+    """n BLS12_G2MUL calls in one pass: data is n x 288 bytes; returns ([status name] * n, n x 256 output bytes)."""
+    return _eth_evm_ecop_batch("bls12381_g2mul", data)
+
+
+def eth_evm_ecops_last_timing() -> dict:
+    """The kernel time (ms, CUDA events) of the calling thread's last call of the curve addition / multiplication entries above;
+    0 when that call did no device work."""
+    v = ctypes.c_float(0)
+    _lib.load().ctt_b200_eth_evm_ecops_last_timing(ctypes.byref(v))
+    return {"ms_kernel": v.value}
+
+
 class CtSpan(ctypes.Structure):
     """ctt_span: {byte* data; size_t len} (reference include/constantine/protocols/ethereum_bls_signatures.h:64)."""
     _fields_ = [("data", ctypes.c_void_p), ("len", ctypes.c_size_t)]
