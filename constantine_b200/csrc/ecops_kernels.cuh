@@ -162,24 +162,25 @@ static __global__ void __launch_bounds__(THREADS) k_evm_mul(const uint8_t* __res
 // The calling thread's last kernel time of any of the curve-operation entries (ms, CUDA events; 0 for n = 0)
 inline float& last_ms() { static thread_local float t = 0; return t; }
 
-// n records on stream s: one copy in, one kernel, one copy of outputs and statuses back; returns the kernel's time (ms)
-template <class W, bool MUL>
-float run_batch(cudaStream_t s, uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t n) {
-  constexpr size_t PT = 2 * W::FBYTES, IN = MUL ? PT + 32 : 2 * PT;
+using RecordKernel = void (*)(const uint8_t*, size_t, uint8_t*, uint8_t*);
+
+// n records of in_bytes on stream s through kernel k (one thread per record, out_bytes of output and one status each): one copy in,
+// one kernel, one copy of outputs and statuses back; returns the kernel's time (ms)
+inline float run_records(cudaStream_t s, RecordKernel k, size_t in_bytes, size_t out_bytes, uint8_t* r, uint8_t* statuses,
+                         const uint8_t* inputs, size_t n) {
   cudaEvent_t ev[2];
   for (auto& e : ev) B200_CUDA_CHECK(cudaEventCreate(&e));
   void *d_in, *d_out, *d_st;
-  B200_CUDA_CHECK(cudaMalloc(&d_in, n * IN + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_out, n * PT + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_in, n * in_bytes + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_out, n * out_bytes + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_st, n + 16));
-  B200_CUDA_CHECK(cudaMemcpyAsync(d_in, inputs, n * IN, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_in, inputs, n * in_bytes, cudaMemcpyHostToDevice, s));
   B200_CUDA_CHECK(cudaEventRecord(ev[0], s));
   const unsigned blocks = (unsigned)((n + THREADS - 1) / THREADS);
-  if (MUL) k_evm_mul<W><<<blocks, THREADS, 0, s>>>((const uint8_t*)d_in, n, (uint8_t*)d_out, (uint8_t*)d_st);
-  else k_evm_add<W><<<blocks, THREADS, 0, s>>>((const uint8_t*)d_in, n, (uint8_t*)d_out, (uint8_t*)d_st);
+  k<<<blocks, THREADS, 0, s>>>((const uint8_t*)d_in, n, (uint8_t*)d_out, (uint8_t*)d_st);
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaEventRecord(ev[1], s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(r, d_out, n * PT, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(r, d_out, n * out_bytes, cudaMemcpyDeviceToHost, s));
   B200_CUDA_CHECK(cudaMemcpyAsync(statuses, d_st, n, cudaMemcpyDeviceToHost, s));
   B200_CUDA_CHECK(cudaStreamSynchronize(s));
   float ms = 0;
@@ -187,6 +188,13 @@ float run_batch(cudaStream_t s, uint8_t* r, uint8_t* statuses, const uint8_t* in
   for (auto& e : ev) cudaEventDestroy(e);
   for (void* p : {d_in, d_out, d_st}) cudaFree(p);
   return ms;
+}
+
+// n curve-operation records: k_evm_mul<W> (P, scalar) or k_evm_add<W> (P, Q) through run_records
+template <class W, bool MUL>
+float run_batch(cudaStream_t s, uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t n) {
+  constexpr size_t PT = 2 * W::FBYTES, IN = MUL ? PT + 32 : 2 * PT;
+  return run_records(s, MUL ? k_evm_mul<W> : k_evm_add<W>, IN, PT, r, statuses, inputs, n);
 }
 
 }  // namespace ecops

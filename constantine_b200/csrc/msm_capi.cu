@@ -318,6 +318,12 @@ int ctt_b200_sm_count(void) {
   return lease.e->sm_count;
 }
 
+extern "C++" {
+namespace b200 {
+int run_test_secp256k1_field_op(int field_id, int op, void* r, const void* a, const void* b, size_t count);   // evm_secp256k1.cu
+}
+}
+
 int ctt_b200_test_field_op(int field_id, int op, void* r, const void* a, const void* b, size_t count) {
   switch (field_id) {
     case 0: return run_test_field_op<Bls12381Fp, 1>(op, r, a, b, count);
@@ -330,6 +336,8 @@ int ctt_b200_test_field_op(int field_id, int op, void* r, const void* a, const v
     case 7: return run_test_field_op<VestaFr, 1>(op, r, a, b, count);
     case 8: return run_test_field_op<Bls12381Fp, 2>(op, r, a, b, count);
     case 9: return run_test_field_op<Bn254SnarksFp, 2>(op, r, a, b, count);
+    case 11:
+    case 12: return run_test_secp256k1_field_op(field_id, op, r, a, b, count);
   }
   return -1;
 }

@@ -389,7 +389,7 @@ def sum_reduce_vartime_parallel(tp, curve, points, length=None, out="jac") -> by
 
 
 EVM_STATUS = ("cttEVM_Success", "cttEVM_InvalidInputSize", "cttEVM_InvalidOutputSize", "cttEVM_IntLargerThanModulus",
-              "cttEVM_PointNotOnCurve", "cttEVM_PointNotInSubgroup", "cttEVM_VerificationFailure")
+              "cttEVM_PointNotOnCurve", "cttEVM_PointNotInSubgroup", "cttEVM_VerificationFailure", "cttEVM_MalformedSignature")
 
 
 def eth_evm_bls12381_g1msm(inputs: bytes, out_len: int = 128):
@@ -618,9 +618,32 @@ def eth_evm_bls12381_g2mul_batch(data: bytes):
     return _eth_evm_ecop_batch("bls12381_g2mul", data)
 
 
+def eth_evm_ecrecover(inputs: bytes, out_len: int = 32):
+    """ECRECOVER (precompile 0x01) through ctt_eth_evm_ecrecover: msg || v || r || s (128 bytes, big-endian) -> (status name, 32
+    bytes). Only bytes 12..31 are written, with the address of the recovered key; bytes 0..11 come back as zeros. An unrecoverable
+    signature succeeds with the zero key's address 0x3f17f1962b36e491b30a40b2405849e597ba5fb5 (see the header for the rules and
+    how they differ from geth)."""
+    return _eth_evm_ecop("ecrecover", inputs, out_len)
+
+
+def eth_evm_ecrecover_batch(data: bytes):
+    """n ECRECOVER calls in one pass (ctt_b200_eth_evm_ecrecover_batch): data is n x 128 bytes; returns ([status name] * n, n x 32
+    output bytes: 12 zero bytes, then the address; all zeros for a malformed record)."""
+    data = bytes(data)
+    if len(data) % 128:
+        raise ValueError("inputs must be a multiple of 128 bytes")
+    n = len(data) // 128
+    r = ctypes.create_string_buffer(max(32 * n, 1))
+    statuses = ctypes.create_string_buffer(max(n, 1))
+    st = _lib.load().ctt_b200_eth_evm_ecrecover_batch(r, statuses, data or b"\0", n)
+    if st != 0:
+        raise ValueError(EVM_STATUS[st])
+    return [EVM_STATUS[b] for b in statuses.raw[:n]], r.raw[:32 * n]
+
+
 def eth_evm_ecops_last_timing() -> dict:
-    """The kernel time (ms, CUDA events) of the calling thread's last call of the curve addition / multiplication entries above;
-    0 when that call did no device work."""
+    """The kernel time (ms, CUDA events) of the calling thread's last call of the curve addition / multiplication or ecrecover
+    entries above; 0 when that call did no device work."""
     v = ctypes.c_float(0)
     _lib.load().ctt_b200_eth_evm_ecops_last_timing(ctypes.byref(v))
     return {"ms_kernel": v.value}
