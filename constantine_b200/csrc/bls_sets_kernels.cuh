@@ -1,6 +1,5 @@
 // Ethereum BLS signature sets on the device (eth_bls.cu, ctt_b200_eth_bls_[batch_]verify_sets): the public keys of every set summed
-// from a resident registry of affine G1 points, optionally blinded, and written as the G1 inputs of the Miller loops; and one final
-// exponentiation per set.
+// from a resident registry of affine G1 points, optionally blinded, and written as the G1 inputs of the Miller loops.
 //
 // Key aggregation runs in two launches. The host cuts every set into chunks of at most SET_CHUNK keys (a chunk never crosses a set
 // boundary) and lists the chunks set by set.
@@ -102,13 +101,6 @@ __global__ void __launch_bounds__(SET_FINISH_THREADS) k_bls_sets_finish(const ui
   uint32_t* dst = g1 + s * stride * (2 * Fq::WORDS);
   store_words(dst, o.x);
   store_words(dst + Fq::WORDS, o.y);
-}
-
-// One thread per product: flags[i] = (final_exponentiation(f[i]) == 1), f: n x 144 words
-__global__ void __launch_bounds__(PAIR_THREADS) k_bls_final_exp_each(const uint32_t* f, size_t n, int* flags) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  flags[i] = final_exponentiation(load_fq12(f + i * GT_WORDS)).is_one() ? 1 : 0;
 }
 
 }  // namespace bls

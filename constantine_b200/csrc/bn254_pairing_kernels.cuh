@@ -22,10 +22,6 @@ using Fq2 = Fp2<Bn254SnarksFp>;
 constexpr int GT_WORDS = 12 * Fq::WORDS;   // 96
 constexpr int PAIR_BYTES = 192;            // P.x, P.y, Q.x_im, Q.x_re, Q.y_im, Q.y_re: 32-byte big-endian integers
 
-// ctt_evm_status (reference constantine/ethereum_evm_precompiles.nim:49-57)
-enum : uint8_t { EVM_SUCCESS = 0, EVM_INVALID_INPUT_SIZE = 1, EVM_INVALID_OUTPUT_SIZE = 2, EVM_INT_LARGER_THAN_MODULUS = 3,
-                 EVM_POINT_NOT_ON_CURVE = 4, EVM_POINT_NOT_IN_SUBGROUP = 5 };
-
 B200_DEV Fq2 mul_xi(const Fq2& a) {   // (a0 + a1 i)(9 + i) = (9 a0 - a1) + (9 a1 + a0) i
   static_assert(XI_C0 == 9 && XI_C1 == 1, "mul_xi is written for xi = 9 + i");
   Fq2 r;
@@ -227,31 +223,31 @@ __device__ __noinline__ uint8_t decode_pair(const uint8_t* src, Aff<Fq>& P, Aff<
   uint32_t w[8];
   Aff<Fq> p;
   load_be32(src, w);
-  if (geq_p(w)) return EVM_INT_LARGER_THAN_MODULUS;
+  if (geq_p(w)) return cttEVM_IntLargerThanModulus;
   p.x = to_mont(w);
   load_be32(src + 32, w);
-  if (geq_p(w)) return EVM_INT_LARGER_THAN_MODULUS;
+  if (geq_p(w)) return cttEVM_IntLargerThanModulus;
   p.y = to_mont(w);
   if (!p.is_inf()) {
     const Fq three = Fq::one().dbl() + Fq::one();
-    if (!(p.y.sqr() == p.x.sqr() * p.x + three)) return EVM_POINT_NOT_ON_CURVE;
+    if (!(p.y.sqr() == p.x.sqr() * p.x + three)) return cttEVM_PointNotOnCurve;
   }
   Fq c[4];   // x_im, x_re, y_im, y_re
 #pragma unroll 1
   for (int k = 0; k < 4; k++) {
     load_be32(src + 64 + 32 * k, w);
-    if (geq_p(w)) return EVM_INT_LARGER_THAN_MODULUS;
+    if (geq_p(w)) return cttEVM_IntLargerThanModulus;
     c[k] = to_mont(w);
   }
   Aff<Fq2> q;
   q.x.c0 = c[1]; q.x.c1 = c[0]; q.y.c0 = c[3]; q.y.c1 = c[2];
   if (!q.is_inf()) {
-    if (!(q.y.sqr() == q.x.sqr() * q.x + fq2_const<Bn254SnarksFp>(BN_TWIST_B, 0))) return EVM_POINT_NOT_ON_CURVE;
-    if (!g2_in_subgroup(q)) return EVM_POINT_NOT_IN_SUBGROUP;
+    if (!(q.y.sqr() == q.x.sqr() * q.x + fq2_const<Bn254SnarksFp>(BN_TWIST_B, 0))) return cttEVM_PointNotOnCurve;
+    if (!g2_in_subgroup(q)) return cttEVM_PointNotInSubgroup;
   }
   P = p;
   Q = q;
-  return EVM_SUCCESS;
+  return cttEVM_Success;
 }
 
 constexpr int DECODE_THREADS = 128;

@@ -37,17 +37,14 @@ namespace ecops {
 
 constexpr int THREADS = 64;
 
-// ctt_evm_status (reference constantine/ethereum_evm_precompiles.nim:49-57), the values a record can get on the device
-enum : uint8_t { EVM_SUCCESS = 0, EVM_INT_LARGER_THAN_MODULUS = 3, EVM_POINT_NOT_ON_CURVE = 4, EVM_POINT_NOT_IN_SUBGROUP = 5 };
-
 template <class W>
 static __device__ __noinline__ uint8_t parse_point(const uint8_t* s, Aff<typename W::F>& p, bool subgroup) {
-  if (!W::load(s, p.x) || !W::load(s + W::FBYTES, p.y)) return EVM_INT_LARGER_THAN_MODULUS;
-  if (p.is_inf()) return EVM_SUCCESS;
-  if (!(p.y.sqr() == p.x.sqr() * p.x + W::b())) return EVM_POINT_NOT_ON_CURVE;
+  if (!W::load(s, p.x) || !W::load(s + W::FBYTES, p.y)) return cttEVM_IntLargerThanModulus;
+  if (p.is_inf()) return cttEVM_Success;
+  if (!(p.y.sqr() == p.x.sqr() * p.x + W::b())) return cttEVM_PointNotOnCurve;
   if constexpr (W::SUBGROUP)
-    if (subgroup && !W::in_subgroup(p)) return EVM_POINT_NOT_IN_SUBGROUP;
-  return EVM_SUCCESS;
+    if (subgroup && !W::in_subgroup(p)) return cttEVM_PointNotInSubgroup;
+  return cttEVM_Success;
 }
 
 template <class W>
@@ -127,8 +124,8 @@ static __global__ void __launch_bounds__(THREADS) k_evm_add(const uint8_t* __res
   Aff<F> p, q, r;
   r.x = F::zero(); r.y = F::zero();
   uint8_t st = parse_point<W>(s, p, false);
-  if (st == EVM_SUCCESS) st = parse_point<W>(s + PT, q, false);
-  if (st == EVM_SUCCESS) {
+  if (st == cttEVM_Success) st = parse_point<W>(s + PT, q, false);
+  if (st == cttEVM_Success) {
     Xyzz<F> acc = Xyzz<F>::from_affine(p);
     xyzz_madd(acc, q);
     r = to_affine(acc);
@@ -148,7 +145,7 @@ static __global__ void __launch_bounds__(THREADS) k_evm_mul(const uint8_t* __res
   Aff<F> p, r;
   r.x = F::zero(); r.y = F::zero();
   const uint8_t st = parse_point<W>(s, p, true);
-  if (st == EVM_SUCCESS) {
+  if (st == cttEVM_Success) {
     uint32_t k[8];
     load_scalar(s + PT, k);
     reduce_scalar<typename W::Fr>(k, W::R_SUBS);

@@ -8,7 +8,7 @@
 //   host:   the status checks, expand_message_xmd of every message (host threads), the serial blinding chain;
 //   engine: sum r_i sigma_i, one G2 MSM (a neutral sum fails the verification, as the reference's Miller accumulator does);
 //   device (one engine lease and stream): hash to G2 (h2c_kernels.cuh), [r_i]PK_i (k_scalar_mul_u64 with a base per item), n + 1 Miller
-//           loops, their tree product and the final exponentiation (pairing_kernels.cuh); one flag comes back.
+//           loops, their product and the final exponentiation (pairing_check.cuh); one flag comes back.
 // aggregate_verify of n pairs (PK_i, m_i) and one signature checks prod_i e(PK_i, H(m_i)) e(-G1, sigma) = 1 the same way, without the
 // blinding and the MSM. ctt_b200_eth_bls_[batch_]verify_sets check signature sets (fast_aggregate_verify per set) with the public keys
 // gathered by index from a resident registry and summed on the device (sets_verify below, bls_sets_kernels.cuh).
@@ -21,6 +21,7 @@
 #include "h2c_kernels.cuh"
 #include "bls_sets_kernels.cuh"
 #include "codec_kernels.cuh"
+#include "pairing_check.cuh"
 #include "eth_kzg_host.hpp"
 #include "host_pairing.hpp"
 #include <algorithm>
@@ -50,9 +51,12 @@ static const char POP_DST[] = "BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_POP_";
 struct Timing { float ms_host = 0, ms_hash = 0, ms_blind = 0, ms_msm = 0, ms_miller = 0, ms_final = 0; };
 static Timing& last_timing() { static thread_local Timing t; return t; }
 
-static double ms_since(std::chrono::steady_clock::time_point t0) {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-}
+// the BLS12-381 pairing of pairing_check.cuh
+struct Pairing {
+  using Tower = bls::Tower;
+  using FinalExp = bls::FinalExp;
+  static constexpr auto miller = bls::k_bls_miller;
+};
 
 static bool all_zero(const uint8_t* p, size_t n) {
   uint8_t o = 0;
@@ -133,30 +137,8 @@ static void read_times(DeviceTimes* times, cudaEvent_t ev[5]) {
 // into the affine G2 points d_out[0..n-1].
 static void hash_device(cudaStream_t s, const uint8_t* uniform, size_t n, void* d_uni, void* d_out) {
   B200_CUDA_CHECK(cudaMemcpyAsync(d_uni, uniform, n * UNIFORM_BYTES, cudaMemcpyHostToDevice, s));
-  bls::k_bls_hash_to_g2<<<(unsigned)((n + bls::H2C_THREADS - 1) / bls::H2C_THREADS), bls::H2C_THREADS, 0, s>>>(
-      (const uint8_t*)d_uni, n, (uint32_t*)d_out);
+  bls::k_bls_hash_to_g2<<<blocks(n, bls::H2C_THREADS), bls::H2C_THREADS, 0, s>>>((const uint8_t*)d_uni, n, (uint32_t*)d_out);
   B200_CUDA_CHECK(cudaGetLastError());
-}
-
-// The Miller loops of the npairs device pairs (d_g1[i], d_g2[i]) into d_f, ev_miller, then levels of the tree product until `until`
-// values remain: 1 gives the whole product, npairs / 2 the products of pairs 2i and 2i + 1. d_f2 is scratch of (npairs + 1) / 2
-// values. Returns the buffer that holds the result (d_f or d_f2).
-static void* miller_product_device(cudaStream_t s, const void* d_g1, const void* d_g2, size_t npairs, size_t until, void* d_f,
-                                   void* d_f2, cudaEvent_t ev_miller) {
-  bls::k_bls_miller<<<(unsigned)((npairs + bls::PAIR_THREADS - 1) / bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>(
-      (const uint32_t*)d_g1, (const uint32_t*)d_g2, npairs, (uint32_t*)d_f);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(ev_miller, s));
-  size_t m = npairs;
-  while (m > until) {
-    const size_t half = (m + 1) / 2;
-    bls::k_bls_fold<<<(unsigned)((half + bls::PAIR_THREADS - 1) / bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>(
-        (const uint32_t*)d_f, m, (uint32_t*)d_f2);
-    B200_CUDA_CHECK(cudaGetLastError());
-    std::swap(d_f, d_f2);
-    m = half;
-  }
-  return d_f;
 }
 
 // The device part of both verifications, on one engine lease and stream. g1: n + 1 affine G1 points (host) -- with blind, the n
@@ -170,14 +152,9 @@ static bool pairing_device(const uint8_t* g1, const uint8_t* uniform, size_t n_h
   cudaStream_t s = E.compute();
   cudaEvent_t ev[5];
   for (auto& e : ev) B200_CUDA_CHECK(cudaEventCreate(&e));
-  void *d_g1, *d_g2, *d_uni = nullptr, *d_r = nullptr, *d_f, *d_f2, *d_gt;
-  int* d_flag;
+  void *d_g1, *d_g2, *d_uni = nullptr, *d_r = nullptr;
   B200_CUDA_CHECK(cudaMalloc(&d_g1, npairs * PK_BYTES + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_g2, npairs * SIG_BYTES + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_f, npairs * 576 + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_f2, ((npairs + 1) / 2) * 576 + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_gt, 576 + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_flag, sizeof(int)));
   B200_CUDA_CHECK(cudaMemcpyAsync(d_g1, g1, npairs * PK_BYTES, cudaMemcpyHostToDevice, s));
   if (n_given) B200_CUDA_CHECK(cudaMemcpyAsync((char*)d_g2 + n_hashed * SIG_BYTES, g2_pts, n_given * SIG_BYTES, cudaMemcpyHostToDevice, s));
   B200_CUDA_CHECK(cudaEventRecord(ev[0], s));
@@ -189,25 +166,18 @@ static bool pairing_device(const uint8_t* g1, const uint8_t* uniform, size_t n_h
   if (blind) {
     B200_CUDA_CHECK(cudaMalloc(&d_r, n_hashed * 8 + 16));
     B200_CUDA_CHECK(cudaMemcpyAsync(d_r, blind, n_hashed * 8, cudaMemcpyHostToDevice, s));
-    k_scalar_mul_u64<bls::Fq><<<(unsigned)((n_hashed + 127) / 128), 128, 0, s>>>((const uint32_t*)d_g1, (const unsigned long long*)d_r,
-                                                                                 n_hashed, (uint32_t*)d_g1, true);
+    k_scalar_mul_u64<bls::Fq><<<blocks(n_hashed, 128), 128, 0, s>>>((const uint32_t*)d_g1, (const unsigned long long*)d_r, n_hashed,
+                                                                    (uint32_t*)d_g1, true);
     B200_CUDA_CHECK(cudaGetLastError());
   }
   B200_CUDA_CHECK(cudaEventRecord(ev[2], s));
-  const void* d_prod = miller_product_device(s, d_g1, d_g2, npairs, 1, d_f, d_f2, ev[3]);
-  bls::k_bls_final_exp<<<1, 32, 0, s>>>((const uint32_t*)d_prod, (uint32_t*)d_gt, d_flag);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(ev[4], s));
-  int flag = 0;
-  B200_CUDA_CHECK(cudaMemcpyAsync(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
-  if (gt_out) B200_CUDA_CHECK(cudaMemcpyAsync(gt_out, d_gt, 576, cudaMemcpyDeviceToHost, s));
-  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  uint8_t ok = 0;
+  pairing_check_device<Pairing>(s, d_g1, d_g2, {0, npairs}, &ok, gt_out, ev[3], ev[4]);
   if (times) read_times(times, ev);
   for (auto& e : ev) cudaEventDestroy(e);
-  cudaFree(d_g1); cudaFree(d_g2); cudaFree(d_f); cudaFree(d_f2); cudaFree(d_gt); cudaFree(d_flag);
-  if (d_uni) cudaFree(d_uni);
-  if (d_r) cudaFree(d_r);
-  return flag != 0;
+  for (void* p : {d_g1, d_g2, d_uni, d_r})
+    if (p) cudaFree(p);
+  return ok != 0;
 }
 
 static bool messages_ok(const Span* messages, size_t n) {
@@ -353,20 +323,17 @@ static uint8_t sets_verify(const ctt_b200_bases* registry, const uint64_t* idx, 
   cudaEvent_t ev[5];
   for (auto& e : ev) B200_CUDA_CHECK(cudaEventCreate(&e));
   const size_t nch = chunks.size();
-  void *d_g1, *d_g2, *d_h, *d_uni, *d_f, *d_f2, *d_gt, *d_idx, *d_chunks, *d_cb, *d_part, *d_r = nullptr;
-  int* d_flags;   // key_inf[n], neutral[n], then the pairing flags (1 in batch mode, n per set)
+  void *d_g1, *d_g2, *d_h, *d_uni, *d_idx, *d_chunks, *d_cb, *d_part, *d_r = nullptr;
+  int* d_flags;   // key_inf[n], then neutral[n]
   B200_CUDA_CHECK(cudaMalloc(&d_g1, npairs * PK_BYTES + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_g2, npairs * SIG_BYTES + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_h, rnd ? 16 : n * SIG_BYTES + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_uni, n * UNIFORM_BYTES + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_f, npairs * 576 + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_f2, ((npairs + 1) / 2) * 576 + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_gt, 576 + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_idx, total * 8 + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_chunks, nch * sizeof(uint4) + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_cb, (n + 1) * 4 + 16));
   B200_CUDA_CHECK(cudaMalloc(&d_part, nch * 4 * 48 + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_flags, 3 * n * sizeof(int) + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_flags, 2 * n * sizeof(int) + 16));
   B200_CUDA_CHECK(cudaMemcpyAsync(d_g1, g1.data(), npairs * PK_BYTES, cudaMemcpyHostToDevice, s));
   if (rnd) {
     B200_CUDA_CHECK(cudaMemcpyAsync((char*)d_g2 + n * SIG_BYTES, g2.data(), SIG_BYTES, cudaMemcpyHostToDevice, s));
@@ -378,7 +345,7 @@ static uint8_t sets_verify(const ctt_b200_bases* registry, const uint64_t* idx, 
   if (total) B200_CUDA_CHECK(cudaMemcpyAsync(d_idx, idx, total * 8, cudaMemcpyHostToDevice, s));
   if (nch) B200_CUDA_CHECK(cudaMemcpyAsync(d_chunks, chunks.data(), nch * sizeof(uint4), cudaMemcpyHostToDevice, s));
   B200_CUDA_CHECK(cudaMemcpyAsync(d_cb, chunk_begin.data(), (n + 1) * 4, cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaMemsetAsync(d_flags, 0, 3 * n * sizeof(int), s));
+  B200_CUDA_CHECK(cudaMemsetAsync(d_flags, 0, 2 * n * sizeof(int), s));
   B200_CUDA_CHECK(cudaEventRecord(ev[0], s));
   if (rnd) hash_device(s, uniform.data(), n, d_uni, d_g2);
   else {
@@ -387,7 +354,7 @@ static uint8_t sets_verify(const ctt_b200_bases* registry, const uint64_t* idx, 
   }
   B200_CUDA_CHECK(cudaEventRecord(ev[1], s));
   if (nch) {
-    bls::k_bls_sets_chunks<<<(unsigned)((nch + bls::SET_CHUNK_THREADS - 1) / bls::SET_CHUNK_THREADS), bls::SET_CHUNK_THREADS, 0, s>>>(
+    bls::k_bls_sets_chunks<<<blocks(nch, bls::SET_CHUNK_THREADS), bls::SET_CHUNK_THREADS, 0, s>>>(
         (const uint32_t*)d_reg, (const unsigned long long*)d_idx, (const uint4*)d_chunks, nch, (uint32_t*)d_part, d_flags);
     B200_CUDA_CHECK(cudaGetLastError());
   }
@@ -396,24 +363,22 @@ static uint8_t sets_verify(const ctt_b200_bases* registry, const uint64_t* idx, 
                                                                          rnd ? 1 : 2, d_flags + n);
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaEventRecord(ev[2], s));
-  const void* d_prod = miller_product_device(s, d_g1, d_g2, npairs, rnd ? 1 : n, d_f, d_f2, ev[3]);
-  if (rnd) bls::k_bls_final_exp<<<1, 32, 0, s>>>((const uint32_t*)d_prod, (uint32_t*)d_gt, d_flags + 2 * n);
-  else bls::k_bls_final_exp_each<<<(unsigned)((n + bls::PAIR_THREADS - 1) / bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>(
-           (const uint32_t*)d_prod, n, d_flags + 2 * n);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(ev[4], s));
-  std::vector<int> flags(3 * n);
-  B200_CUDA_CHECK(cudaMemcpyAsync(flags.data(), d_flags, (rnd ? 2 * n + 1 : 3 * n) * sizeof(int), cudaMemcpyDeviceToHost, s));
+  std::vector<size_t> begin;   // batch: one call of n + 1 pairs; per set: n calls of 2
+  for (size_t b = 0; b <= npairs; b += rnd ? n + 1 : 2) begin.push_back(b);
+  std::vector<uint8_t> ok(begin.size() - 1);
+  pairing_check_device<Pairing>(s, d_g1, d_g2, begin, ok.data(), nullptr, ev[3], ev[4]);
+  std::vector<int> flags(2 * n);
+  B200_CUDA_CHECK(cudaMemcpyAsync(flags.data(), d_flags, 2 * n * sizeof(int), cudaMemcpyDeviceToHost, s));
   B200_CUDA_CHECK(cudaStreamSynchronize(s));
   DeviceTimes dt;
   read_times(&dt, ev);
   for (auto& e : ev) cudaEventDestroy(e);
-  for (void* p : {d_g1, d_g2, d_h, d_uni, d_f, d_f2, d_gt, d_idx, d_chunks, d_cb, d_part, (void*)d_flags}) cudaFree(p);
+  for (void* p : {d_g1, d_g2, d_h, d_uni, d_idx, d_chunks, d_cb, d_part, (void*)d_flags}) cudaFree(p);
   if (d_r) cudaFree(d_r);
   t.ms_hash = dt.ms_hash; t.ms_blind = dt.ms_blind; t.ms_miller = dt.ms_miller; t.ms_final = dt.ms_final;
   last_timing() = t;
 
-  const int *key_inf = flags.data(), *neutral = flags.data() + n, *ok = flags.data() + 2 * n;
+  const int *key_inf = flags.data(), *neutral = flags.data() + n;
   for (size_t i = 0; i < n; i++)
     if (st[i] == Success && key_inf[i]) st[i] = PointAtInfinity;
   if (rnd) {

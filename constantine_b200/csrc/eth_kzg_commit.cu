@@ -113,10 +113,6 @@ static void batch_affine(const HP* p, size_t count, Fp* xy) {
 struct Timing { float ms_host = 0, ms_quotient = 0; };
 static Timing& last_timing() { static thread_local Timing t; return t; }
 
-static double ms_since(std::chrono::steady_clock::time_point t0) {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-}
-
 // proofs[j] (and y[j] if y is not null) for n validated blobs and their opening points
 static void prove(const Context* k, uint8_t* proofs, uint8_t* y, const uint8_t* blobs, const std::vector<OpeningArgs>& args, float ms_host) {
   const size_t n = args.size();
@@ -335,6 +331,7 @@ static unsigned char verify_blobs(const Context* k, const uint8_t* blobs, const 
 }  // namespace b200
 
 using namespace b200::kzg;
+using b200::ms_since;
 
 extern "C" {
 

@@ -11,8 +11,8 @@
 // A single entry writes r only when it returns Success. A failed call or element of a batch reads zeros.
 //
 // Per batch, on one engine lease and stream: pairing checks run the decoder (statuses, curve and subgroup checks), one Miller loop
-// per pair (k_bls_miller), the levels of each call's product and one final exponentiation per call (tower.cuh); maps run one kernel
-// that writes the wire output and the statuses. There is no CPU path.
+// per pair (k_bls_miller), the levels of each call's product and one final exponentiation per call (pairing_check.cuh); maps run
+// one kernel that writes the wire output and the statuses. There is no CPU path.
 //
 // EIP-2537 BLS12_G1ADD, G2ADD, G1MUL and G2MUL: ctt_eth_evm_bls12381_g{1,2}{add,mul} (the reference's names and prototypes; Nim
 // source constantine/ethereum_evm_precompiles.nim:628-892), and batch entries of many independent calls. The input length (256 /
@@ -24,161 +24,50 @@
 #include "../../include/ctt_b200_msm.h"
 #include "msm_hooks.cuh"
 #include "eip2537_kernels.cuh"
-#include <algorithm>
-#include <chrono>
+#include "pairing_check.cuh"
 #include <cstring>
-#include <vector>
 
 namespace b200 {
 namespace evmbls {
 
 using namespace eip2537;
-constexpr size_t G1_BYTES = 2 * 48, G2_BYTES = 4 * 48, GT_BYTES = 4 * bls::GT_WORDS;
 
 struct Timing { float ms_host = 0, ms_decode = 0, ms_map = 0, ms_miller = 0, ms_final = 0; };
 static Timing& last_timing() { static thread_local Timing t; return t; }
 
-static unsigned blocks(size_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
-
-static double ms_since(std::chrono::steady_clock::time_point t0) {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-}
-
-// npairs wire pairs; call c owns pairs begin[c] .. begin[c + 1] - 1 (each call at least one). pair_status receives the status of
-// every pair, ok[c] the flag of call c.
-static void pairing_device(const uint8_t* wire, size_t npairs, const std::vector<size_t>& begin, uint8_t* pair_status, uint8_t* ok,
-                           Timing& t) {
-  const size_t ncalls = begin.size() - 1;
-  std::vector<size_t> call_of(npairs);
-  size_t longest = 0;
-  for (size_t c = 0; c < ncalls; c++) {
-    std::fill(call_of.begin() + begin[c], call_of.begin() + begin[c + 1], c);
-    longest = std::max(longest, begin[c + 1] - begin[c]);
-  }
-  EngineLease lease = acquire_engine();
-  Engine& E = *lease.e;
-  cudaStream_t s = E.compute();
-  cudaEvent_t ev[4];
-  for (auto& e : ev) B200_CUDA_CHECK(cudaEventCreate(&e));
-  void *d_wire, *d_g1, *d_g2, *d_st, *d_f, *d_call, *d_begin, *d_ok;
-  B200_CUDA_CHECK(cudaMalloc(&d_wire, npairs * PAIR_BYTES + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_g1, npairs * G1_BYTES + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_g2, npairs * G2_BYTES + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_st, npairs + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_f, npairs * GT_BYTES + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_call, npairs * sizeof(size_t) + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_begin, (ncalls + 1) * sizeof(size_t) + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_ok, ncalls + 16));
-  B200_CUDA_CHECK(cudaMemcpyAsync(d_call, call_of.data(), npairs * sizeof(size_t), cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(d_begin, begin.data(), (ncalls + 1) * sizeof(size_t), cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(d_wire, wire, npairs * PAIR_BYTES, cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(ev[0], s));
-  k_eip2537_decode<<<blocks(npairs, DECODE_THREADS), DECODE_THREADS, 0, s>>>((const uint8_t*)d_wire, npairs, (uint32_t*)d_g1,
-                                                                             (uint32_t*)d_g2, (uint8_t*)d_st);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(ev[1], s));
-  bls::k_bls_miller<<<blocks(npairs, bls::PAIR_THREADS), bls::PAIR_THREADS, 0, s>>>((const uint32_t*)d_g1, (const uint32_t*)d_g2,
-                                                                                    npairs, (uint32_t*)d_f);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(ev[2], s));
-  for (size_t stride = 1; stride < longest; stride *= 2) {
-    k_pairing_fold<bls::Tower><<<blocks(npairs, PAIRING_THREADS), PAIRING_THREADS, 0, s>>>((uint32_t*)d_f, (const size_t*)d_call,
-                                                                                           (const size_t*)d_begin, npairs, stride);
-    B200_CUDA_CHECK(cudaGetLastError());
-  }
-  k_pairing_final_exp<bls::Tower, bls::FinalExp><<<blocks(ncalls, PAIRING_THREADS), PAIRING_THREADS, 0, s>>>(
-      (const uint32_t*)d_f, (const size_t*)d_begin, ncalls, (uint8_t*)d_ok, nullptr);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(ev[3], s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(ok, d_ok, ncalls, cudaMemcpyDeviceToHost, s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(pair_status, d_st, npairs, cudaMemcpyDeviceToHost, s));
-  B200_CUDA_CHECK(cudaStreamSynchronize(s));
-  cudaEventElapsedTime(&t.ms_decode, ev[0], ev[1]);
-  cudaEventElapsedTime(&t.ms_miller, ev[1], ev[2]);
-  cudaEventElapsedTime(&t.ms_final, ev[2], ev[3]);
-  for (auto& e : ev) cudaEventDestroy(e);
-  for (void* p : {d_wire, d_g1, d_g2, d_st, d_f, d_call, d_begin, d_ok}) cudaFree(p);
-}
-
-// k calls, call i = inputs[offsets[i], offsets[i + 1]); r: k x 32 bytes, statuses: k bytes
-static uint8_t pairing_check_batch(uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t inputs_len, const size_t* offsets,
-                                   size_t k) {
-  if (k == 0) return EVM_SUCCESS;
-  if (!r || !statuses || !inputs || !offsets) return EVM_INVALID_INPUT_SIZE;
-  for (size_t i = 0; i < k; i++)
-    if (offsets[i + 1] < offsets[i]) return EVM_INVALID_INPUT_SIZE;
-  if (offsets[k] > inputs_len) return EVM_INVALID_INPUT_SIZE;
-
-  Timing t;
-  const auto t0 = std::chrono::steady_clock::now();
-  memset(r, 0, 32 * k);
-  std::vector<size_t> dev_calls, begin(1, 0);   // the calls that need a pairing, and their first pairs in `wire`
-  for (size_t i = 0; i < k; i++) {
-    const size_t len = offsets[i + 1] - offsets[i];
-    if (len == 0 || len % PAIR_BYTES) { statuses[i] = EVM_INVALID_INPUT_SIZE; continue; }
-    statuses[i] = EVM_SUCCESS;
-    dev_calls.push_back(i);
-    begin.push_back(begin.back() + len / PAIR_BYTES);
-  }
-  if (!dev_calls.empty()) {
-    const size_t npairs = begin.back();
-    std::vector<uint8_t> wire(npairs * PAIR_BYTES), pair_status(npairs), ok(dev_calls.size());
-    for (size_t c = 0; c < dev_calls.size(); c++)
-      memcpy(&wire[begin[c] * PAIR_BYTES], inputs + offsets[dev_calls[c]], (begin[c + 1] - begin[c]) * PAIR_BYTES);
-    t.ms_host = (float)ms_since(t0);
-    pairing_device(wire.data(), npairs, begin, pair_status.data(), ok.data(), t);
-    for (size_t c = 0; c < dev_calls.size(); c++) {
-      const size_t i = dev_calls[c];
-      for (size_t j = begin[c]; j < begin[c + 1]; j++)
-        if (pair_status[j] != EVM_SUCCESS) { statuses[i] = pair_status[j]; break; }
-      if (statuses[i] == EVM_SUCCESS && ok[c]) r[32 * i + 31] = 1;
-    }
-  } else {
-    t.ms_host = (float)ms_since(t0);
-  }
-  last_timing() = t;
-  return EVM_SUCCESS;
-}
+// the BLS12-381 pairing of pairing_check.cuh, with the EIP-2537 wire format
+struct Pairing {
+  using Tower = bls::Tower;
+  using FinalExp = bls::FinalExp;
+  static constexpr auto miller = bls::k_bls_miller;
+  static constexpr auto decode = k_eip2537_decode;
+  static constexpr int DECODE_THREADS = eip2537::DECODE_THREADS;
+  static constexpr size_t PAIR_BYTES = eip2537::PAIR_BYTES;
+  static constexpr bool EMPTY_IS_ONE = false;   // EIP-2537 has no empty pairing check
+};
 
 // n maps of `in_bytes` -> `out_bytes` (64 -> 128 on G1, 128 -> 256 on G2)
 static uint8_t map_batch(bool g2, uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t n) {
-  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return EVM_INVALID_INPUT_SIZE;
+  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return cttEVM_InvalidInputSize;
   Timing t;
-  if (n == 0) { last_timing() = t; return EVM_SUCCESS; }
-  const size_t in_bytes = g2 ? 128 : 64, out_bytes = 2 * in_bytes;
-  EngineLease lease = acquire_engine();
-  Engine& E = *lease.e;
-  cudaStream_t s = E.compute();
-  cudaEvent_t ev[2];
-  for (auto& e : ev) B200_CUDA_CHECK(cudaEventCreate(&e));
-  void *d_in, *d_out, *d_st;
-  B200_CUDA_CHECK(cudaMalloc(&d_in, n * in_bytes + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_out, n * out_bytes + 16));
-  B200_CUDA_CHECK(cudaMalloc(&d_st, n + 16));
-  B200_CUDA_CHECK(cudaMemcpyAsync(d_in, inputs, n * in_bytes, cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaEventRecord(ev[0], s));
-  if (g2) k_eip2537_map_g2<<<blocks(n, MAP_THREADS), MAP_THREADS, 0, s>>>((const uint8_t*)d_in, n, (uint8_t*)d_out, (uint8_t*)d_st);
-  else k_eip2537_map_g1<<<blocks(n, MAP_THREADS), MAP_THREADS, 0, s>>>((const uint8_t*)d_in, n, (uint8_t*)d_out, (uint8_t*)d_st);
-  B200_CUDA_CHECK(cudaGetLastError());
-  B200_CUDA_CHECK(cudaEventRecord(ev[1], s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(r, d_out, n * out_bytes, cudaMemcpyDeviceToHost, s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(statuses, d_st, n, cudaMemcpyDeviceToHost, s));
-  B200_CUDA_CHECK(cudaStreamSynchronize(s));
-  cudaEventElapsedTime(&t.ms_map, ev[0], ev[1]);
-  for (auto& e : ev) cudaEventDestroy(e);
-  for (void* p : {d_in, d_out, d_st}) cudaFree(p);
+  if (n) {
+    const size_t in_bytes = g2 ? 128 : 64;
+    EngineLease lease = acquire_engine();
+    t.ms_map = ecops::run_records(lease.e->compute(), g2 ? k_eip2537_map_g2 : k_eip2537_map_g1, in_bytes, 2 * in_bytes, r, statuses,
+                                  inputs, n);
+  }
   last_timing() = t;
-  return EVM_SUCCESS;
+  return cttEVM_Success;
 }
 
 // the single map entries: input size, then output size, then the batch of one; r is written only on success
 static uint8_t map_one(bool g2, uint8_t* r, size_t r_len, const uint8_t* inputs, size_t inputs_len) {
   const size_t in_bytes = g2 ? 128 : 64, out_bytes = 2 * in_bytes;
-  if (inputs_len != in_bytes || !inputs) return EVM_INVALID_INPUT_SIZE;
-  if (r_len != out_bytes || !r) return EVM_INVALID_OUTPUT_SIZE;
+  if (inputs_len != in_bytes || !inputs) return cttEVM_InvalidInputSize;
+  if (r_len != out_bytes || !r) return cttEVM_InvalidOutputSize;
   uint8_t out[256], status;
   map_batch(g2, out, &status, inputs, 1);
-  if (status == EVM_SUCCESS) memcpy(r, out, out_bytes);
+  if (status == cttEVM_Success) memcpy(r, out, out_bytes);
   return status;
 }
 
@@ -214,9 +103,9 @@ constexpr size_t ECOP_IN[] = {256, 512, 160, 288}, ECOP_OUT[] = {128, 256, 128, 
 
 // n records of ECOP_IN[op] bytes -> n x ECOP_OUT[op] bytes and n statuses
 static uint8_t ecop_batch(EcOp op, uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t n) {
-  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return EVM_INVALID_INPUT_SIZE;
+  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return cttEVM_InvalidInputSize;
   ecops::last_ms() = 0;
-  if (n == 0) return EVM_SUCCESS;
+  if (n == 0) return cttEVM_Success;
   EngineLease lease = acquire_engine();
   cudaStream_t s = lease.e->compute();
   float ms = 0;
@@ -227,17 +116,17 @@ static uint8_t ecop_batch(EcOp op, uint8_t* r, uint8_t* statuses, const uint8_t*
     case G2MUL: ms = ecops::run_batch<G2Wire, true>(s, r, statuses, inputs, n); break;
   }
   ecops::last_ms() = ms;
-  return EVM_SUCCESS;
+  return cttEVM_Success;
 }
 
 // the single entries: input size, then output size, then the batch of one; r is written only on success
 static uint8_t ecop_one(EcOp op, uint8_t* r, size_t r_len, const uint8_t* inputs, size_t inputs_len) {
   ecops::last_ms() = 0;
-  if (inputs_len != ECOP_IN[op] || !inputs) return EVM_INVALID_INPUT_SIZE;
-  if (r_len != ECOP_OUT[op] || !r) return EVM_INVALID_OUTPUT_SIZE;
+  if (inputs_len != ECOP_IN[op] || !inputs) return cttEVM_InvalidInputSize;
+  if (r_len != ECOP_OUT[op] || !r) return cttEVM_InvalidOutputSize;
   uint8_t out[256], status;
   ecop_batch(op, out, &status, inputs, 1);
-  if (status == EVM_SUCCESS) memcpy(r, out, ECOP_OUT[op]);
+  if (status == cttEVM_Success) memcpy(r, out, ECOP_OUT[op]);
   return status;
 }
 
@@ -250,13 +139,13 @@ extern "C" {
 
 // reference include/constantine/protocols/ethereum_evm_precompiles.h (eth_evm_bls12381_pairingcheck)
 ctt_evm_status ctt_eth_evm_bls12381_pairingcheck(byte* r, size_t r_len, const byte* inputs, size_t inputs_len) {
-  if (r_len != 32 || !r) return (ctt_evm_status)eip2537::EVM_INVALID_OUTPUT_SIZE;
-  if (!inputs && inputs_len) return (ctt_evm_status)eip2537::EVM_INVALID_INPUT_SIZE;
+  if (r_len != 32 || !r) return cttEVM_InvalidOutputSize;
+  if (!inputs && inputs_len) return cttEVM_InvalidInputSize;
   static const uint8_t none = 0;
   const size_t offsets[2] = {0, inputs_len};
   uint8_t out[32], status;
-  evmbls::pairing_check_batch(out, &status, inputs ? inputs : &none, inputs_len, offsets, 1);
-  if (status == eip2537::EVM_SUCCESS) memcpy(r, out, 32);
+  pairing_check_batch<evmbls::Pairing>(evmbls::last_timing(), out, &status, inputs ? inputs : &none, inputs_len, offsets, 1);
+  if (status == cttEVM_Success) memcpy(r, out, 32);
   return (ctt_evm_status)status;
 }
 
@@ -272,7 +161,7 @@ ctt_evm_status ctt_eth_evm_bls12381_map_fp2_to_g2(byte* r, size_t r_len, const b
 
 ctt_evm_status ctt_b200_eth_evm_bls12381_pairingcheck_batch(byte* r, byte* statuses, const byte* inputs, size_t inputs_len,
                                                             const size_t* offsets, size_t k) {
-  return (ctt_evm_status)evmbls::pairing_check_batch(r, statuses, inputs, inputs_len, offsets, k);
+  return (ctt_evm_status)pairing_check_batch<evmbls::Pairing>(evmbls::last_timing(), r, statuses, inputs, inputs_len, offsets, k);
 }
 
 ctt_evm_status ctt_b200_eth_evm_bls12381_map_fp_to_g1_batch(byte* r, byte* statuses, const byte* inputs, size_t n) {

@@ -30,7 +30,6 @@ namespace b200 {
 namespace evmk1 {
 
 constexpr size_t IN_BYTES = 128, OUT_BYTES = 32;
-enum : uint8_t { EVM_SUCCESS = 0, EVM_INVALID_INPUT_SIZE = 1, EVM_INVALID_OUTPUT_SIZE = 2, EVM_MALFORMED_SIGNATURE = 7 };
 
 B200_DEV bool is_zero8(const uint32_t* w) {
   uint32_t o = 0;
@@ -137,7 +136,7 @@ static __global__ void __launch_bounds__(ecops::THREADS) k_evm_ecrecover(const u
   if (!well_formed) {
     o[0] = make_uint4(0, 0, 0, 0);
     o[1] = make_uint4(0, 0, 0, 0);
-    status[i] = EVM_MALFORMED_SIGNATURE;
+    status[i] = cttEVM_MalformedSignature;
     return;
   }
   const Aff<FpK1> q = recover(s, vb == 1 || vb == 28);
@@ -150,27 +149,27 @@ static __global__ void __launch_bounds__(ecops::THREADS) k_evm_ecrecover(const u
   keccak::keccak256_64(msg, h);
   o[0] = make_uint4(0, 0, 0, h[3]);
   o[1] = make_uint4(h[4], h[5], h[6], h[7]);
-  status[i] = EVM_SUCCESS;
+  status[i] = cttEVM_Success;
 }
 
 // n records of 128 bytes -> n x 32 bytes and n statuses
 static uint8_t ecrecover_batch(uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t n) {
-  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return EVM_INVALID_INPUT_SIZE;
+  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return cttEVM_InvalidInputSize;
   ecops::last_ms() = 0;
-  if (n == 0) return EVM_SUCCESS;
+  if (n == 0) return cttEVM_Success;
   EngineLease lease = acquire_engine();
   ecops::last_ms() = ecops::run_records(lease.e->compute(), k_evm_ecrecover, IN_BYTES, OUT_BYTES, r, statuses, inputs, n);
-  return EVM_SUCCESS;
+  return cttEVM_Success;
 }
 
 // the single entry: the input size, then the output size; only r[12..31] is written, and only on success
 static uint8_t ecrecover_one(uint8_t* r, size_t r_len, const uint8_t* inputs, size_t inputs_len) {
   ecops::last_ms() = 0;
-  if (inputs_len != IN_BYTES || !inputs) return EVM_INVALID_INPUT_SIZE;
-  if (r_len != OUT_BYTES || !r) return EVM_INVALID_OUTPUT_SIZE;
+  if (inputs_len != IN_BYTES || !inputs) return cttEVM_InvalidInputSize;
+  if (r_len != OUT_BYTES || !r) return cttEVM_InvalidOutputSize;
   uint8_t out[OUT_BYTES], status;
   ecrecover_batch(out, &status, inputs, 1);
-  if (status == EVM_SUCCESS) memcpy(r + 12, out + 12, OUT_BYTES - 12);
+  if (status == cttEVM_Success) memcpy(r + 12, out + 12, OUT_BYTES - 12);
   return status;
 }
 

@@ -9,6 +9,7 @@
 // reference constantine/math/arithmetic/limbs_montgomery.nim:180-217 for CIOS), written for
 // 64-bit limbs with unsigned __int128.
 #pragma once
+#include <chrono>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
@@ -301,4 +302,10 @@ inline void xyzz_to_prj(const HXyzz<T>& p, T& X, T& Y, T& Z) {
 }
 
 }  // namespace host
+
+// milliseconds on the host clock since t0, for the entries' last_timing splits
+inline double ms_since(std::chrono::steady_clock::time_point t0) {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+
 }  // namespace b200

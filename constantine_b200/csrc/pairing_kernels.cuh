@@ -1,6 +1,6 @@
 // BLS12-381 optimal ate pairing on the device: Fp6 / Fp12 over the device Fp2 (the shared tower of tower.cuh), the Miller loop with
-// T in homogeneous projective coordinates and sparse line products, the tree product of the per-pair values and the final
-// exponentiation.
+// T in homogeneous projective coordinates and sparse line products, and the final exponentiation (the products and the final
+// exponentiation kernels are tower.cuh's, run by pairing_check.cuh).
 //
 // Tower: the one of host_pairing.hpp (Fp6 = Fp2[v] / (v^3 - xi), xi = 1 + i, Fp12 = Fp6[w] / (w^2 - v)), so the GT bytes compare
 // directly with the host. Lines are the host's, scaled by factors in Fp2, which the final exponentiation removes.
@@ -132,9 +132,7 @@ B200_DEV Fq12 miller_loop(const Aff<Fq>& P, const Aff<Fq2>& Q) {
   return f.conj();
 }
 
-B200_DEV Fq12 load_fq12(const uint32_t* src) { return b200::load_fq12<Tower>(src); }
-
-constexpr int PAIR_THREADS = 64;
+constexpr int PAIR_THREADS = PAIRING_THREADS;
 
 // One pair per thread: f_i = miller_loop(P_i, Q_i). g1: n affine G1 points, g2: n affine G2 points (ABI layout), f: n x 144 words.
 static __global__ void __launch_bounds__(PAIR_THREADS) k_bls_miller(const uint32_t* g1, const uint32_t* g2, size_t n, uint32_t* f) {
@@ -143,23 +141,6 @@ static __global__ void __launch_bounds__(PAIR_THREADS) k_bls_miller(const uint32
   Aff<Fq> P; load_words_rw(P.x, g1 + i * 2 * Fq::WORDS); load_words_rw(P.y, g1 + i * 2 * Fq::WORDS + Fq::WORDS);
   Aff<Fq2> Q; load_words_rw(Q.x, g2 + i * 2 * Fq2::WORDS); load_words_rw(Q.y, g2 + i * 2 * Fq2::WORDS + Fq2::WORDS);
   store_fq12(f + i * GT_WORDS, miller_loop(P, Q));
-}
-
-// One level of the tree product: out[i] = in[2i] * in[2i + 1] (in[2i] alone when 2i + 1 = n). out may not alias in.
-static __global__ void __launch_bounds__(PAIR_THREADS) k_bls_fold(const uint32_t* in, size_t n, uint32_t* out) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (2 * i >= n) return;
-  Fq12 a = load_fq12(in + 2 * i * GT_WORDS);
-  if (2 * i + 1 < n) a = fq12_mul(a, load_fq12(in + (2 * i + 1) * GT_WORDS));
-  store_fq12(out + i * GT_WORDS, a);
-}
-
-// One thread: gt = final_exponentiation(f), flag = (gt == 1)
-static __global__ void __launch_bounds__(32) k_bls_final_exp(const uint32_t* f, uint32_t* gt, int* flag) {
-  if (threadIdx.x != 0) return;
-  const Fq12 r = final_exponentiation(load_fq12(f));
-  store_fq12(gt, r);
-  *flag = r.is_one() ? 1 : 0;
 }
 
 }  // namespace bls

@@ -417,9 +417,8 @@ def eth_evm_bn254_ecpairingcheck(inputs: bytes, out_len: int = 32):
     return EVM_STATUS[st], r.raw[:out_len]
 
 
-def eth_evm_bn254_ecpairingcheck_batch(calls) -> list:
-    """Many independent ecPairing calls in one pass (ctt_b200_eth_evm_bn254_ecpairingcheck_batch): calls is a sequence of byte
-    strings; returns [(status name, 32 output bytes)] in the same order, as the single entry gives them per call."""
+def _eth_evm_pairingcheck_batch(name, calls) -> list:
+    """Many independent pairing-check calls in one pass through the offsets-based batch entry `name`."""
     calls = [bytes(c) for c in calls]
     k = len(calls)
     if k == 0:
@@ -430,11 +429,31 @@ def eth_evm_bn254_ecpairingcheck_batch(calls) -> list:
     data = b"".join(calls) or b"\0"
     r = ctypes.create_string_buffer(32 * k)
     statuses = ctypes.create_string_buffer(k)
-    st = _lib.load().ctt_b200_eth_evm_bn254_ecpairingcheck_batch(r, statuses, data, offsets[k], offsets, k)
+    st = getattr(_lib.load(), name)(r, statuses, data, offsets[k], offsets, k)
     if st != 0:
         raise ValueError(EVM_STATUS[st])
     raw = r.raw
     return [(EVM_STATUS[statuses.raw[i]], raw[32 * i:32 * i + 32]) for i in range(k)]
+
+
+def _eth_evm_records_batch(name, data, in_bytes, out_bytes):
+    """n fixed-size records of in_bytes in one pass through the batch entry `name`: ([status name] * n, n x out_bytes)."""
+    data = bytes(data)
+    if len(data) % in_bytes:
+        raise ValueError("inputs must be a multiple of %d bytes" % in_bytes)
+    n = len(data) // in_bytes
+    r = ctypes.create_string_buffer(max(out_bytes * n, 1))
+    statuses = ctypes.create_string_buffer(max(n, 1))
+    st = getattr(_lib.load(), name)(r, statuses, data or b"\0", n)
+    if st != 0:
+        raise ValueError(EVM_STATUS[st])
+    return [EVM_STATUS[b] for b in statuses.raw[:n]], r.raw[:out_bytes * n]
+
+
+def eth_evm_bn254_ecpairingcheck_batch(calls) -> list:
+    """Many independent ecPairing calls in one pass (ctt_b200_eth_evm_bn254_ecpairingcheck_batch): calls is a sequence of byte
+    strings; returns [(status name, 32 output bytes)] in the same order, as the single entry gives them per call."""
+    return _eth_evm_pairingcheck_batch("ctt_b200_eth_evm_bn254_ecpairingcheck_batch", calls)
 
 
 def eth_evm_bn254_last_timing() -> dict:
@@ -458,21 +477,7 @@ def eth_evm_bls12381_pairingcheck(inputs: bytes, out_len: int = 32):
 def eth_evm_bls12381_pairingcheck_batch(calls) -> list:
     """Many independent BLS12_PAIRING_CHECK calls in one pass (ctt_b200_eth_evm_bls12381_pairingcheck_batch): calls is a sequence of
     byte strings; returns [(status name, 32 output bytes)] in the same order, as the single entry gives them per call."""
-    calls = [bytes(c) for c in calls]
-    k = len(calls)
-    if k == 0:
-        return []
-    offsets = (ctypes.c_size_t * (k + 1))()
-    for i, c in enumerate(calls):
-        offsets[i + 1] = offsets[i] + len(c)
-    data = b"".join(calls) or b"\0"
-    r = ctypes.create_string_buffer(32 * k)
-    statuses = ctypes.create_string_buffer(k)
-    st = _lib.load().ctt_b200_eth_evm_bls12381_pairingcheck_batch(r, statuses, data, offsets[k], offsets, k)
-    if st != 0:
-        raise ValueError(EVM_STATUS[st])
-    raw = r.raw
-    return [(EVM_STATUS[statuses.raw[i]], raw[32 * i:32 * i + 32]) for i in range(k)]
+    return _eth_evm_pairingcheck_batch("ctt_b200_eth_evm_bls12381_pairingcheck_batch", calls)
 
 
 def _eth_evm_bls12381_map(name, inputs, out_len):
@@ -494,29 +499,16 @@ def eth_evm_bls12381_map_fp2_to_g2(inputs: bytes, out_len: int = 256):
     return _eth_evm_bls12381_map("ctt_eth_evm_bls12381_map_fp2_to_g2", inputs, out_len)
 
 
-def _eth_evm_bls12381_map_batch(name, data, in_bytes):
-    data = bytes(data)
-    if len(data) % in_bytes:
-        raise ValueError("inputs must be a multiple of %d bytes" % in_bytes)
-    n = len(data) // in_bytes
-    r = ctypes.create_string_buffer(max(2 * in_bytes * n, 1))
-    statuses = ctypes.create_string_buffer(max(n, 1))
-    st = getattr(_lib.load(), name)(r, statuses, data or b"\0", n)
-    if st != 0:
-        raise ValueError(EVM_STATUS[st])
-    return [EVM_STATUS[b] for b in statuses.raw[:n]], r.raw[:2 * in_bytes * n]
-
-
 def eth_evm_bls12381_map_fp_to_g1_batch(data: bytes):
     """n maps to G1 in one pass (ctt_b200_eth_evm_bls12381_map_fp_to_g1_batch): data is n x 64 bytes; returns ([status name] * n,
     n x 128 output bytes), a failed element's output zeros."""
-    return _eth_evm_bls12381_map_batch("ctt_b200_eth_evm_bls12381_map_fp_to_g1_batch", data, 64)
+    return _eth_evm_records_batch("ctt_b200_eth_evm_bls12381_map_fp_to_g1_batch", data, 64, 128)
 
 
 def eth_evm_bls12381_map_fp2_to_g2_batch(data: bytes):
     """n maps to G2 in one pass (ctt_b200_eth_evm_bls12381_map_fp2_to_g2_batch): data is n x 128 bytes; returns ([status name] * n,
     n x 256 output bytes), a failed element's output zeros."""
-    return _eth_evm_bls12381_map_batch("ctt_b200_eth_evm_bls12381_map_fp2_to_g2_batch", data, 128)
+    return _eth_evm_records_batch("ctt_b200_eth_evm_bls12381_map_fp2_to_g2_batch", data, 128, 256)
 
 
 def eth_evm_bls12381_last_timing() -> dict:
@@ -574,17 +566,7 @@ def eth_evm_bls12381_g2mul(inputs: bytes, out_len: int = 256):
 
 
 def _eth_evm_ecop_batch(name, data):
-    in_bytes, out_bytes = ECOPS[name]
-    data = bytes(data)
-    if len(data) % in_bytes:
-        raise ValueError("inputs must be a multiple of %d bytes" % in_bytes)
-    n = len(data) // in_bytes
-    r = ctypes.create_string_buffer(max(out_bytes * n, 1))
-    statuses = ctypes.create_string_buffer(max(n, 1))
-    st = getattr(_lib.load(), "ctt_b200_eth_evm_" + name + "_batch")(r, statuses, data or b"\0", n)
-    if st != 0:
-        raise ValueError(EVM_STATUS[st])
-    return [EVM_STATUS[b] for b in statuses.raw[:n]], r.raw[:out_bytes * n]
+    return _eth_evm_records_batch("ctt_b200_eth_evm_" + name + "_batch", data, *ECOPS[name])
 
 
 def eth_evm_bn254_g1add_batch(data: bytes):
@@ -629,16 +611,7 @@ def eth_evm_ecrecover(inputs: bytes, out_len: int = 32):
 def eth_evm_ecrecover_batch(data: bytes):
     """n ECRECOVER calls in one pass (ctt_b200_eth_evm_ecrecover_batch): data is n x 128 bytes; returns ([status name] * n, n x 32
     output bytes: 12 zero bytes, then the address; all zeros for a malformed record)."""
-    data = bytes(data)
-    if len(data) % 128:
-        raise ValueError("inputs must be a multiple of 128 bytes")
-    n = len(data) // 128
-    r = ctypes.create_string_buffer(max(32 * n, 1))
-    statuses = ctypes.create_string_buffer(max(n, 1))
-    st = _lib.load().ctt_b200_eth_evm_ecrecover_batch(r, statuses, data or b"\0", n)
-    if st != 0:
-        raise ValueError(EVM_STATUS[st])
-    return [EVM_STATUS[b] for b in statuses.raw[:n]], r.raw[:32 * n]
+    return _eth_evm_records_batch("ctt_b200_eth_evm_ecrecover_batch", data, 128, 32)
 
 
 def eth_evm_ecops_last_timing() -> dict:
