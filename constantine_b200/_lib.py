@@ -175,6 +175,14 @@ def load():
     lib.ctt_b200_eth_kzg_verify_blob_kzg_proof_batch.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_kzg_last_verify_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 5
     lib.ctt_b200_eth_kzg_last_verify_timing.restype = None
+    lib.ctt_b200_eth_kzg_verify_kzg_proofs.argtypes = [vp, vp, vp, vp, vp, vp, sz]
+    lib.ctt_b200_eth_kzg_verify_kzg_proofs.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_evm_kzg_point_evaluation.argtypes = [vp, vp, sz, vp, sz]
+    lib.ctt_b200_eth_evm_kzg_point_evaluation.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_evm_kzg_point_evaluation_batch.argtypes = [vp, vp, vp, vp, sz]
+    lib.ctt_b200_eth_evm_kzg_point_evaluation_batch.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_kzg_last_point_eval_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 4
+    lib.ctt_b200_eth_kzg_last_point_eval_timing.restype = None
     ub = ctypes.c_uint8
     lib.ctt_eth_bls_batch_verify.argtypes = [vp, vp, vp, sz, vp]
     lib.ctt_eth_bls_batch_verify.restype = ub

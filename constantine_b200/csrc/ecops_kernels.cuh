@@ -15,6 +15,8 @@
 // Scalar multiplication: k mod r by conditional subtraction, then a signed fixed window of 4 bits over a per-thread table of
 // [1..8]P (XYZZ): Booth digits d_i = b(4i-1) + b(4i) + 2 b(4i+1) + 4 b(4i+2) - 8 b(4i+3) in [-8, 8], read from the top 5 bits of
 // the scalar as it shifts left by 4. k < r < 2^255, so bit 255 is zero and 64 digits are exact.
+// joint_mul (u1 G + u2 R for a fixed G) serves ECRECOVER (evm_secp256k1.cu) and the KZG opening check of the point-evaluation
+// precompile (evm_bls12381_precompiles.cu).
 // Not constant time: every input of a precompile is public.
 #pragma once
 #include "ec.cuh"
@@ -80,6 +82,53 @@ B200_DEV void reduce_scalar(uint32_t* w, int subs) {
 #pragma unroll
     for (int i = 0; i < 8; i++) w[i] = t[i];
   }
+}
+
+// Booth digit of bits 4i + 3 .. 4i - 1 from the top 5 bits of the shifting scalar, in [-8, 8]
+B200_DEV int booth(const uint32_t* k) {
+  const uint32_t v = k[7] >> 27;
+  return (int)((v + 1) >> 1) - 16 * (int)(v >> 4);
+}
+B200_DEV void shl4(uint32_t* k) {
+#pragma unroll
+  for (int w = 7; w > 0; w--) k[w] = (k[w] << 4) | (k[w - 1] >> 28);
+  k[0] <<= 4;
+}
+
+// u1 G + u2 R for 256-bit u1, u2 (8 little-endian words each, consumed), G the curve's fixed generator and R affine (finite or
+// infinity): one joint loop of signed 4-bit digits with shared doublings. Bit 255 may be set (secp256k1's n > 2^255): it is the
+// extra top digit 64 (0 or 1), then digits 63..0. Additions: R's from a per-thread XYZZ table of [1..8]R, G's mixed from the
+// constant affine table that Gt::multiple(d) reads ([d]G for d in [-8, 8] \ {0}). ec.cuh's group law is exact at infinity, P = Q
+// and P = -Q, which u1 G = +-u2 R can reach.
+template <class T, class Gt>
+static __device__ __noinline__ Xyzz<T> joint_mul(const Aff<T>& r, uint32_t* u1, uint32_t* u2) {
+  Xyzz<T> tab[8];   // [1..8]R
+  tab[0] = Xyzz<T>::from_affine(r);
+#pragma unroll 1
+  for (int j = 1; j < 8; j++) {
+    tab[j] = tab[j - 1];
+    xyzz_madd(tab[j], r);
+  }
+  Xyzz<T> acc = Xyzz<T>::inf();
+  if (u1[7] >> 31) xyzz_madd(acc, Gt::multiple(1));
+  if (u2[7] >> 31) xyzz_add(acc, tab[0]);
+#pragma unroll 1
+  for (int i = 63; i >= 0; i--) {
+    if (!acc.is_inf()) {
+#pragma unroll 1
+      for (int j = 0; j < 4; j++) acc = xyzz_dbl(acc);
+    }
+    const int d1 = booth(u1), d2 = booth(u2);
+    if (d1 != 0) xyzz_madd(acc, Gt::multiple(d1));
+    if (d2 != 0) {
+      Xyzz<T> t = tab[(d2 < 0 ? -d2 : d2) - 1];
+      if (d2 < 0) t.y = t.y.neg();
+      xyzz_add(acc, t);
+    }
+    shl4(u1);
+    shl4(u2);
+  }
+  return acc;
 }
 
 // [k]P, k < 2^255 (8 little-endian words, consumed), P affine (finite or infinity)

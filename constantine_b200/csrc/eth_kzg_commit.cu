@@ -327,6 +327,56 @@ static unsigned char verify_blobs(const Context* k, const uint8_t* blobs, const 
   return pairing_neg_g2(k, res[0], k->g2[1], res[1], tm);
 }
 
+// ---- EIP-4844 single openings on the device: verify_kzg_proofs and the point-evaluation precompile ------------------------------
+// host time of the last call (packing, statuses) and its device phases (ctt_b200_eth_kzg_last_point_eval_timing)
+struct PointEvalTiming { float ms_host = 0, ms_records = 0, ms_miller = 0, ms_final = 0; };
+static PointEvalTiming& last_point_eval_timing() { static thread_local PointEvalTiming t; return t; }
+
+constexpr size_t POINT_EVAL_BYTES = 192;   // versioned_hash(32) | z(32) | y(32) | commitment(48) | proof(48)
+static_assert(sizeof(G2Aff) == 192, "G2Aff is the device's affine G2 layout");
+
+// n > 0 records -> statuses[i], verify_kzg_proof's status for record i (after the versioned hash when check_hash, a mismatch giving
+// VerificationFailure): the first failing check's, else Success or VerificationFailure from its pairing check. k has the G2 setup.
+static void point_eval(const Context* k, const uint8_t* records, size_t n, bool check_hash, uint8_t* statuses, double ms_host) {
+  G2Aff g2[2] = {k->g2[1], k->g2[0]};   // [tau]G2, -G2
+  g2[1].y = g2[1].y.neg();
+  std::vector<uint8_t> ok(n);
+  PointEvalTimes times;
+  point_eval_device(g2, records, n, check_hash, statuses, ok.data(), &times);
+  const auto t0 = std::chrono::steady_clock::now();
+  for (size_t i = 0; i < n; i++)
+    if (statuses[i] == Success && !ok[i]) statuses[i] = VerificationFailure;
+  PointEvalTiming& t = last_point_eval_timing();
+  t.ms_host = (float)(ms_host + ms_since(t0));
+  t.ms_records = times.ms_records;
+  t.ms_miller = times.ms_miller;
+  t.ms_final = times.ms_final;
+}
+
+// The precompile's output on success: FIELD_ELEMENTS_PER_BLOB and the BLS12-381 scalar field's modulus, 32 big-endian bytes each
+static constexpr uint8_t POINT_EVAL_OUTPUT[64] = {
+    0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0x10, 0x00,
+    0x73, 0xed, 0xa7, 0x53, 0x29, 0x9d, 0x7d, 0x48, 0x33, 0x39, 0xd8, 0x08, 0x09, 0xa1, 0xd8, 0x05,
+    0x53, 0xbd, 0xa4, 0x02, 0xff, 0xfe, 0x5b, 0xfe, 0xff, 0xff, 0xff, 0xff, 0x00, 0x00, 0x00, 0x01};
+
+// n precompile calls of 192 bytes -> n x 64 bytes (zeros for a failed call) and n ctt_evm_status values
+static uint8_t evm_point_eval_batch(const Context* k, uint8_t* r, uint8_t* statuses, const uint8_t* inputs, size_t n) {
+  if (n >= (size_t(1) << 31) || (n && (!r || !statuses || !inputs))) return cttEVM_InvalidInputSize;
+  if (!k || k->g2.size() != DAS_L_G2) return cttEVM_VerificationFailure;
+  last_point_eval_timing() = PointEvalTiming();
+  if (n == 0) return cttEVM_Success;
+  point_eval(k, inputs, n, true, statuses, 0.0);
+  const auto t0 = std::chrono::steady_clock::now();
+  for (size_t i = 0; i < n; i++) {
+    const bool pass = statuses[i] == Success;
+    statuses[i] = pass ? cttEVM_Success : cttEVM_VerificationFailure;
+    if (pass) memcpy(r + 64 * i, POINT_EVAL_OUTPUT, 64);
+    else memset(r + 64 * i, 0, 64);
+  }
+  last_point_eval_timing().ms_host += (float)ms_since(t0);
+  return cttEVM_Success;
+}
+
 }  // namespace kzg
 }  // namespace b200
 
@@ -675,6 +725,55 @@ unsigned char ctt_b200_eth_kzg_verify_blob_kzg_proof_batch(const ctt_b200_eth_kz
   if (n == 0) return (unsigned char)Success;
   if (!blobs || !commitments || !proofs || !secure_random_bytes) return (unsigned char)InputsLengthsMismatch;
   return verify_blobs(k, blobs, commitments, proofs, n, secure_random_bytes);
+}
+
+// n independent verify_kzg_proof checks on the device (statuses[i] as ctt_b200_eth_kzg_verify_kzg_proof returns it for index i), packed
+// into the point-evaluation precompile's record layout with the versioned hash left unchecked
+unsigned char ctt_b200_eth_kzg_verify_kzg_proofs(const ctt_b200_eth_kzg_context* ctx, unsigned char* statuses, const unsigned char* commitments,
+                                                 const unsigned char* zs, const unsigned char* ys, const unsigned char* proofs, size_t n) {
+  const Context* k = reinterpret_cast<const Context*>(ctx);
+  if (!k || k->g2.size() != DAS_L_G2) return (unsigned char)VerificationFailure;
+  if (n >= (size_t(1) << 31) || (n && (!statuses || !commitments || !zs || !ys || !proofs))) return (unsigned char)InputsLengthsMismatch;
+  last_point_eval_timing() = PointEvalTiming();
+  if (n == 0) return (unsigned char)Success;
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<uint8_t> rec(POINT_EVAL_BYTES * n, 0);
+  for (size_t i = 0; i < n; i++) {
+    uint8_t* d = &rec[POINT_EVAL_BYTES * i];
+    memcpy(d + 32, zs + 32 * i, 32);
+    memcpy(d + 64, ys + 32 * i, 32);
+    memcpy(d + 96, commitments + 48 * i, 48);
+    memcpy(d + 144, proofs + 48 * i, 48);
+  }
+  point_eval(k, rec.data(), n, false, statuses, ms_since(t0));
+  return (unsigned char)Success;
+}
+
+// the last verify_kzg_proofs / point-evaluation call of the calling thread: host packing and statuses, and the device phases
+void ctt_b200_eth_kzg_last_point_eval_timing(float* ms_host, float* ms_records, float* ms_miller, float* ms_final) {
+  const PointEvalTiming& t = last_point_eval_timing();
+  if (ms_host) *ms_host = t.ms_host;
+  if (ms_records) *ms_records = t.ms_records;
+  if (ms_miller) *ms_miller = t.ms_miller;
+  if (ms_final) *ms_final = t.ms_final;
+}
+
+// reference eth_evm_kzg_point_evaluation (constantine/ethereum_evm_precompiles.nim:1245-1297) with this library's context: the input
+// size, then the output size, then the context, then the versioned hash and verify_kzg_proof on the device; r only on success
+ctt_evm_status ctt_b200_eth_evm_kzg_point_evaluation(const ctt_b200_eth_kzg_context* ctx, byte* r, size_t r_len, const byte* inputs,
+                                                     size_t inputs_len) {
+  if (inputs_len != POINT_EVAL_BYTES || !inputs) return cttEVM_InvalidInputSize;
+  if (r_len != 64 || !r) return cttEVM_InvalidOutputSize;
+  uint8_t out[64], status;
+  const uint8_t rc = evm_point_eval_batch(reinterpret_cast<const Context*>(ctx), out, &status, inputs, 1);
+  if (rc != cttEVM_Success) return (ctt_evm_status)rc;
+  if (status == cttEVM_Success) memcpy(r, out, 64);
+  return (ctt_evm_status)status;
+}
+
+ctt_evm_status ctt_b200_eth_evm_kzg_point_evaluation_batch(const ctt_b200_eth_kzg_context* ctx, byte* r, byte* statuses, const byte* inputs,
+                                                           size_t n) {
+  return (ctt_evm_status)evm_point_eval_batch(reinterpret_cast<const Context*>(ctx), r, statuses, inputs, n);
 }
 
 // the last verification of the calling thread, of either family (verify_cell_kzg_proof_batch, verify_kzg_proof, verify_blob_kzg_proof,

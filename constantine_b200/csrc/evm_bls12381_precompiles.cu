@@ -20,11 +20,17 @@
 // coordinate in range, then all zeros is infinity, else on the curve (twist), and for the multiplications in G1 (G2). The additions
 // do not check the subgroup. The scalar is any 256-bit value, reduced mod r. Per batch one engine lease and stream, one kernel
 // (ecops_kernels.cuh) that writes the wire output and the statuses.
+//
+// The device half of the EIP-4844 single-opening check (kzg_device.hpp point_eval_device), behind verify_kzg_proofs and the
+// POINT_EVALUATION precompile (eth_kzg_commit.cu): one thread per 192-byte record (k_kzg_point_eval), then one pairing check of
+// two pairs per record through the same Miller, fold and final-exponentiation kernels as BLS12_PAIRING_CHECK.
 #define CTT_B200_BUILDING_LIBRARY
 #include "../../include/ctt_b200_msm.h"
 #include "msm_hooks.cuh"
 #include "eip2537_kernels.cuh"
+#include "kzg_device.hpp"
 #include "pairing_check.cuh"
+#include "sha256.cuh"
 #include <cstring>
 
 namespace b200 {
@@ -131,6 +137,167 @@ static uint8_t ecop_one(EcOp op, uint8_t* r, size_t r_len, const uint8_t* inputs
 }
 
 }  // namespace evmbls
+
+// ---- EIP-4844 single openings ------------------------------------------------------------------------------------------------
+namespace kzg {
+
+using bls::Fq;
+using bls::Fq2;
+
+// A record: versioned_hash(32) | z(32) | y(32) | commitment(48) | proof(48), the precompile's input; every field 16-byte aligned.
+constexpr size_t RECORD_BYTES = 192;
+constexpr uint8_t KZG_FAILURE = 1, KZG_SCALAR_GEQ_R = 4;   // cttEthKzg_VerificationFailure, cttEthKzg_ScalarLargerThanCurveOrder
+
+// the constant table [1..8]G1 of ecops::joint_mul (bls_constants.cuh): the j-th point, negated for d < 0 (d in [-8, 8] \ {0})
+struct G1Table {
+  static B200_DEV Aff<Fq> multiple(int d) {
+    const uint32_t* t = bls::G1_TABLE + 2 * Fq::WORDS * ((d < 0 ? -d : d) - 1);
+    Aff<Fq> g;
+#pragma unroll
+    for (int w = 0; w < Fq::WORDS; w++) { g.x.set_word(w, __ldg(t + w)); g.y.set_word(w, __ldg(t + Fq::WORDS + w)); }
+    if (d < 0) g.y = g.y.neg();
+    return g;
+  }
+};
+
+// 0x01 || sha256(commitment)[1:] equals the record's versioned hash
+B200_DEV bool versioned_hash_matches(const uint8_t* s) {
+  const uint4* q = reinterpret_cast<const uint4*>(s);
+  uint32_t m[12], h[8];
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    const uint4 v = __ldg(q + 6 + k);   // the commitment, bytes 96..143
+    m[4 * k] = __byte_perm(v.x, 0, 0x0123);
+    m[4 * k + 1] = __byte_perm(v.y, 0, 0x0123);
+    m[4 * k + 2] = __byte_perm(v.z, 0, 0x0123);
+    m[4 * k + 3] = __byte_perm(v.w, 0, 0x0123);
+  }
+  sha256::sha256_48(m, h);
+  h[0] = (h[0] & 0x00FFFFFFu) | 0x01000000u;
+  const uint4 a = __ldg(q), b = __ldg(q + 1);
+  const uint32_t vh[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+  uint32_t diff = 0;
+#pragma unroll
+  for (int k = 0; k < 8; k++) diff |= __byte_perm(vh[k], 0, 0x0123) ^ h[k];
+  return diff == 0;
+}
+
+// A 48-byte compressed G1 point -> affine Montgomery (infinity as (0, 0)) and the status of the host's decompress_g1 + subgroup
+// test: the byte-level checks of k_bls_decode_g1, then codec::g1_decode; codec statuses 1..4 are cttEthKzg 5..8, a valid infinity
+// (codec 5) is a point.
+static __device__ __noinline__ uint8_t decode_g1(const uint8_t* s, Aff<Fq>& p) {
+  p.x = Fq::zero();
+  p.y = Fq::zero();
+  uint32_t w[12];
+  codec::load_be48(s, w);
+  const uint32_t flags = w[11] >> 24;
+  int st;
+  if (!(flags & 0x80)) st = codec::CODEC_INVALID_ENCODING;
+  else if (flags & 0x40) st = (flags & 0x3F) || !codec::rest_zero(w) ? codec::CODEC_INVALID_ENCODING : codec::CODEC_OK;
+  else {
+    w[11] &= 0x1FFFFFFFu;
+    st = codec::geq_p(w) ? codec::CODEC_GEQ_MODULUS : codec::g1_decode(w, (flags & 0x20) != 0, p.x, p.y);
+  }
+  return st == codec::CODEC_OK ? 0 : (uint8_t)(st + 4);
+}
+
+// w < r for 8 little-endian words
+B200_DEV bool below_r(const uint32_t* w) {
+  p_sub_cc(w[0], Bls12381Fr::P(0));
+#pragma unroll
+  for (int i = 1; i < 8; i++) p_subc_cc(w[i], Bls12381Fr::P(i));
+  return p_subc(0, 0) != 0;
+}
+
+// w = -w mod r for w < r
+B200_DEV void neg_mod_r(uint32_t* w) {
+  uint32_t o = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) o |= w[i];
+  if (o == 0) return;
+  w[0] = p_sub_cc(Bls12381Fr::P(0), w[0]);
+#pragma unroll
+  for (int i = 1; i < 8; i++) w[i] = p_subc_cc(Bls12381Fr::P(i), w[i]);
+}
+
+// src: n records; g2_pair: [tau]G2 then -G2 (affine Montgomery, 48 words each). Record i's checks, in verify_kzg_proof's order after
+// the versioned hash (when check_hash): commitment, z < r, y < r, proof; status[i] = 0 when they pass, else the first failing one's
+// cttEthKzg status (1 for the hash). Then Q = C + [z]pi - [y]G1 and the record's two pairs: (pi, [tau]G2) at 2i, (Q, -G2) at 2i + 1,
+// in k_bls_miller's layout. A failed record's G1 points are infinity, so its pairing product is 1 and its status decides.
+static __global__ void __launch_bounds__(ecops::THREADS) k_kzg_point_eval(const uint8_t* __restrict__ src, size_t n, bool check_hash,
+                                                                        const uint32_t* __restrict__ g2_pair, uint32_t* g1, uint32_t* g2,
+                                                                        uint8_t* status) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint8_t* s = src + RECORD_BYTES * i;
+  Aff<Fq> c, pi, q;
+  q.x = Fq::zero();
+  q.y = Fq::zero();
+  uint32_t z[8], y[8];
+  uint8_t st = check_hash && !versioned_hash_matches(s) ? KZG_FAILURE : 0;
+  if (st == 0) st = decode_g1(s + 96, c);
+  if (st == 0) {
+    ecops::load_scalar(s + 32, z);
+    if (!below_r(z)) st = KZG_SCALAR_GEQ_R;
+  }
+  if (st == 0) {
+    ecops::load_scalar(s + 64, y);
+    if (!below_r(y)) st = KZG_SCALAR_GEQ_R;
+  }
+  if (st == 0) st = decode_g1(s + 144, pi);
+  if (st == 0) {
+    neg_mod_r(y);
+    Xyzz<Fq> acc = ecops::joint_mul<Fq, G1Table>(pi, y, z);   // [-y]G1 + [z]pi
+    xyzz_madd(acc, c);
+    q = to_affine(acc);
+  } else {
+    pi.x = Fq::zero();
+    pi.y = Fq::zero();
+  }
+  uint32_t* o = g1 + 2 * i * 2 * Fq::WORDS;
+  store_words(o, pi.x);
+  store_words(o + Fq::WORDS, pi.y);
+  store_words(o + 2 * Fq::WORDS, q.x);
+  store_words(o + 3 * Fq::WORDS, q.y);
+  uint32_t* o2 = g2 + 2 * i * 2 * Fq2::WORDS;
+#pragma unroll 4
+  for (int k = 0; k < 4 * Fq2::WORDS; k++) o2[k] = __ldg(g2_pair + k);
+  status[i] = st;
+}
+
+void point_eval_device(const void* g2_pair, const uint8_t* records, size_t n, bool check_hash, uint8_t* status, uint8_t* ok,
+                       PointEvalTimes* times) {
+  constexpr size_t G1_BYTES = 2 * Fq::WORDS * 4, G2_BYTES = 2 * Fq2::WORDS * 4;
+  EngineLease lease = acquire_engine();
+  cudaStream_t s = lease.e->compute();
+  cudaEvent_t ev[4];
+  for (auto& e : ev) B200_CUDA_CHECK(cudaEventCreate(&e));
+  void *d_in, *d_pair, *d_g1, *d_g2, *d_st;
+  B200_CUDA_CHECK(cudaMalloc(&d_in, n * RECORD_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_pair, 2 * G2_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_g1, 2 * n * G1_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_g2, 2 * n * G2_BYTES + 16));
+  B200_CUDA_CHECK(cudaMalloc(&d_st, n + 16));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_in, records, n * RECORD_BYTES, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d_pair, g2_pair, 2 * G2_BYTES, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaEventRecord(ev[0], s));
+  k_kzg_point_eval<<<blocks(n, ecops::THREADS), ecops::THREADS, 0, s>>>((const uint8_t*)d_in, n, check_hash, (const uint32_t*)d_pair,
+                                                                        (uint32_t*)d_g1, (uint32_t*)d_g2, (uint8_t*)d_st);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(ev[1], s));
+  std::vector<size_t> begin(n + 1);
+  for (size_t c = 0; c <= n; c++) begin[c] = 2 * c;
+  pairing_check_device<evmbls::Pairing>(s, d_g1, d_g2, begin, ok, nullptr, ev[2], ev[3]);
+  B200_CUDA_CHECK(cudaMemcpyAsync(status, d_st, n, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  cudaEventElapsedTime(&times->ms_records, ev[0], ev[1]);
+  cudaEventElapsedTime(&times->ms_miller, ev[1], ev[2]);
+  cudaEventElapsedTime(&times->ms_final, ev[2], ev[3]);
+  for (auto& e : ev) cudaEventDestroy(e);
+  for (void* p : {d_in, d_pair, d_g1, d_g2, d_st}) cudaFree(p);
+}
+
+}  // namespace kzg
 }  // namespace b200
 
 using namespace b200;

@@ -38,60 +38,17 @@ B200_DEV bool is_zero8(const uint32_t* w) {
   return o == 0;
 }
 
-// j-th point of the constant table [1..8]G, negated for d < 0 (d in [-8, 8] \ {0})
-B200_DEV Aff<FpK1> g_multiple(int d) {
-  const uint32_t* t = k1::G_TABLE + 16 * ((d < 0 ? -d : d) - 1);
-  Aff<FpK1> g;
+// the constant table [1..8]G of ecops::joint_mul: the j-th point, negated for d < 0 (d in [-8, 8] \ {0})
+struct GTable {
+  static B200_DEV Aff<FpK1> multiple(int d) {
+    const uint32_t* t = k1::G_TABLE + 16 * ((d < 0 ? -d : d) - 1);
+    Aff<FpK1> g;
 #pragma unroll
-  for (int w = 0; w < 8; w++) { g.x.l[w] = __ldg(t + w); g.y.l[w] = __ldg(t + 8 + w); }
-  if (d < 0) g.y = g.y.neg();
-  return g;
-}
-
-// Booth digit of bits 4i + 3 .. 4i - 1 from the top 5 bits of the shifting scalar, in [-8, 8]
-B200_DEV int booth(const uint32_t* k) {
-  const uint32_t v = k[7] >> 27;
-  return (int)((v + 1) >> 1) - 16 * (int)(v >> 4);
-}
-B200_DEV void shl4(uint32_t* k) {
-#pragma unroll
-  for (int w = 7; w > 0; w--) k[w] = (k[w] << 4) | (k[w - 1] >> 28);
-  k[0] <<= 4;
-}
-
-// u1 G + u2 R for u1, u2 < n (8 little-endian words each, consumed), R affine and finite: one joint loop of signed 4-bit digits with
-// shared doublings. n > 2^255, so bit 255 may be set: it is the extra top digit 64 (0 or 1), then digits 63..0. Additions: R's
-// from a per-thread XYZZ table of [1..8]R, G's mixed from the constant affine table. ec.cuh's group law is exact at infinity,
-// P = Q and P = -Q, which u1 G = +-u2 R can reach.
-static __device__ __noinline__ Xyzz<FpK1> joint_mul(const Aff<FpK1>& r, uint32_t* u1, uint32_t* u2) {
-  Xyzz<FpK1> tab[8];   // [1..8]R
-  tab[0] = Xyzz<FpK1>::from_affine(r);
-#pragma unroll 1
-  for (int j = 1; j < 8; j++) {
-    tab[j] = tab[j - 1];
-    xyzz_madd(tab[j], r);
+    for (int w = 0; w < 8; w++) { g.x.l[w] = __ldg(t + w); g.y.l[w] = __ldg(t + 8 + w); }
+    if (d < 0) g.y = g.y.neg();
+    return g;
   }
-  Xyzz<FpK1> acc = Xyzz<FpK1>::inf();
-  if (u1[7] >> 31) xyzz_madd(acc, g_multiple(1));
-  if (u2[7] >> 31) xyzz_add(acc, tab[0]);
-#pragma unroll 1
-  for (int i = 63; i >= 0; i--) {
-    if (!acc.is_inf()) {
-#pragma unroll 1
-      for (int j = 0; j < 4; j++) acc = xyzz_dbl(acc);
-    }
-    const int d1 = booth(u1), d2 = booth(u2);
-    if (d1 != 0) xyzz_madd(acc, g_multiple(d1));
-    if (d2 != 0) {
-      Xyzz<FpK1> t = tab[(d2 < 0 ? -d2 : d2) - 1];
-      if (d2 < 0) t.y = t.y.neg();
-      xyzz_add(acc, t);
-    }
-    shl4(u1);
-    shl4(u2);
-  }
-  return acc;
-}
+};
 
 // the recovered key of one well-formed record (affine; (0, 0) when there is none)
 static __device__ __noinline__ Aff<FpK1> recover(const uint8_t* s, bool odd) {
@@ -118,7 +75,7 @@ static __device__ __noinline__ Aff<FpK1> recover(const uint8_t* s, bool odd) {
   k1::fr_mul(u1, m, ri);
   k1::fr_neg(u1, u1);
   k1::fr_mul(u2, sc, ri);
-  return to_affine(joint_mul(R, u1, u2));
+  return to_affine(ecops::joint_mul<FpK1, GTable>(R, u1, u2));   // R is finite
 }
 
 // src: n records of 128 bytes; out: n x 32 bytes (12 zero bytes, then the 20-byte address; all zeros on MalformedSignature)

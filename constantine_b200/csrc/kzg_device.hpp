@@ -129,5 +129,17 @@ int verify_blob_device(const void* d_roots, const BlobVerifyBatch& vb, const std
                        const std::function<int(const uint8_t*)>& decide, const OpeningArgs* args, const uint64_t* r_mont,
                        host::HXyzz<host::HFp<Bls12381Fp>>* out, VerifyTimes* times);
 
+// ---- EIP-4844 single openings: verify_kzg_proofs and the point-evaluation precompile (evm_bls12381_precompiles.cu) ------------
+struct PointEvalTimes {
+  float ms_records = 0, ms_miller = 0, ms_final = 0;   // CUDA events: k_kzg_point_eval; the Miller loops; the folds + final exps
+};
+
+// n > 0 records of 192 bytes, versioned_hash(32) | z(32) | y(32) | commitment(48) | proof(48). status[i]: 0 when record i passes its
+// checks (the versioned hash when check_hash, then verify_kzg_proof's: commitment, z < r, y < r, proof), else the cttEthKzg status
+// of the first failing one (1 for the versioned hash). ok[i]: e(pi, [tau]G2) e(C + [z]pi - [y]G1, -G2) = 1, or the record failed
+// a check. g2_pair: [tau]G2 then -G2, two affine Montgomery G2 points (host_pairing.hpp G2Aff). One engine lease and stream.
+void point_eval_device(const void* g2_pair, const uint8_t* records, size_t n, bool check_hash, uint8_t* status, uint8_t* ok,
+                       PointEvalTimes* times);
+
 }  // namespace kzg
 }  // namespace b200

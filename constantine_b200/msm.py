@@ -1097,6 +1097,58 @@ class EthKzgContext:
                                                                       _buf(b"".join(proofs) or b"\0"), n, _buf(bytes(secure_random_bytes)))
         return self._verify_status(rc)
 
+    def verify_kzg_proofs(self, commitments, zs, ys, proofs) -> list:
+        """n independent verify_kzg_proof checks in one device pass (ctt_b200_eth_kzg_verify_kzg_proofs): the list of the n statuses,
+        each what verify_kzg_proof's C entry returns for that index (0 true, 1 false, 4-8 an input that does not decode). Not a
+        random linear combination: every index has its own pairing check."""
+        self._need_g2("verify_kzg_proofs")
+        cols = [[bytes(x) for x in col] for col in (commitments, zs, ys, proofs)]
+        n = len(cols[0])
+        if any(len(col) != n for col in cols):
+            raise ValueError("commitments, zs, ys and proofs differ in length: %s" % [len(col) for col in cols])
+        for name, col, size in zip(("commitment", "z", "y", "proof"), cols, (48, 32, 32, 48)):
+            for x in col:
+                self._check_len(name, x, size)
+        statuses = ctypes.create_string_buffer(max(n, 1))
+        rc = _lib.load().ctt_b200_eth_kzg_verify_kzg_proofs(self._h, statuses, *[_buf(b"".join(col) or b"\0") for col in cols], n)
+        if rc != 0:
+            raise ValueError(rc)
+        return list(statuses.raw[:n])
+
+    # The EIP-4844 POINT_EVALUATION precompile (0x0a; reference constantine/ethereum_evm_precompiles.nim:1245-1297) on this context:
+    # versioned_hash(32) | z(32) | y(32) | commitment(48) | proof(48) -> FIELD_ELEMENTS_PER_BLOB || r, 32 big-endian bytes each.
+    def eth_evm_kzg_point_evaluation(self, inputs, out_len: int = 64):
+        """One call through ctt_b200_eth_evm_kzg_point_evaluation: (status name, out_len bytes); the output is written only on
+        success (zeros otherwise)."""
+        self._need_g2("eth_evm_kzg_point_evaluation")
+        inputs = bytes(inputs)
+        r = ctypes.create_string_buffer(max(out_len, 1))
+        st = _lib.load().ctt_b200_eth_evm_kzg_point_evaluation(self._h, r, out_len, inputs or b"\0", len(inputs))
+        return EVM_STATUS[st], r.raw[:out_len]
+
+    def eth_evm_kzg_point_evaluation_batch(self, data):
+        """n calls in one pass (ctt_b200_eth_evm_kzg_point_evaluation_batch): data is n x 192 bytes; returns ([status name] * n, n x 64
+        output bytes), a failed call's output zeros."""
+        self._need_g2("eth_evm_kzg_point_evaluation_batch")
+        data = bytes(data)
+        if len(data) % 192:
+            raise ValueError("inputs must be a multiple of 192 bytes")
+        n = len(data) // 192
+        r = ctypes.create_string_buffer(max(64 * n, 1))
+        statuses = ctypes.create_string_buffer(max(n, 1))
+        st = _lib.load().ctt_b200_eth_evm_kzg_point_evaluation_batch(self._h, r, statuses, data or b"\0", n)
+        if st != 0:
+            raise ValueError(EVM_STATUS[st])
+        return [EVM_STATUS[b] for b in statuses.raw[:n]], r.raw[:64 * n]
+
+    @staticmethod
+    def last_point_eval_timing() -> dict:
+        """Host packing and statuses, the record kernel, the Miller loops and the products with final exponentiations (ms, CUDA
+        events) of the calling thread's last verify_kzg_proofs or point-evaluation call."""
+        v = [ctypes.c_float(0) for _ in range(4)]
+        _lib.load().ctt_b200_eth_kzg_last_point_eval_timing(*[ctypes.byref(x) for x in v])
+        return dict(zip(("ms_host", "ms_records", "ms_miller", "ms_final"), (x.value for x in v)))
+
     @staticmethod
     def last_verify_timing() -> dict:
         """Host checks + challenges, device decode, scalar kernels, bank MSM (CUDA events) and host pairing time (ms) of the calling

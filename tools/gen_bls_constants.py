@@ -18,6 +18,8 @@ Nothing here is copied from a table: every constant is computed from the curve.
   - beta, the cube root of unity of Fp for which phi(x, y) = (beta x, y) acts on G1 as [-u^2] (u = -X_ABS): the G1 subgroup test of
     Scott (eprint 2021/1130) checks phi(P) = [-u^2]P. Of the two primitive cube roots exactly one does; the generator asserts it on
     the G1 generator. It goes to constantine_b200/csrc/codec_constants.cuh (the decoders of codec_g1.cuh / codec_kernels.cuh).
+  - [1..8]G1, affine, the constant table of the joint scalar multiplication (ecops::joint_mul) in the KZG opening check of the
+    point-evaluation precompile.
 """
 import json
 import os
@@ -601,6 +603,23 @@ def emit(name, elems, words_of=fp2_words):
     return "\n".join(lines)
 
 
+def g1_table():
+    """[1..8]G1 (affine, finite) as x then y, the table the signed 4-bit digits of ecops::joint_mul read."""
+    pts = [g1_mul(j, G1_GEN) for j in range(1, 9)]
+    assert all(p is not None and (p[1] * p[1] - p[0] ** 3 - 4) % P == 0 for p in pts)
+    return [c for p in pts for c in p]
+
+
+def emit_global(name, elems):
+    """A table that threads index with different values: global memory (read through __ldg), not the constant bank."""
+    words = [w for e in elems for w in mont_words(e)]
+    lines = ["static __device__ const uint32_t %s[%d] = {" % (name, len(words))]
+    for k in range(0, len(words), 8):
+        lines.append("    " + ", ".join("0x%08xu" % w for w in words[k:k + 8]) + ",")
+    lines.append("};")
+    return "\n".join(lines)
+
+
 def header_text():
     xn, xd, yn, yd = select_isogeny(load_rfc_vectors())
     g1n, g1d, g1yn, g1yd = select_g1_isogeny(load_rfc_g1_vectors())
@@ -627,6 +646,8 @@ def header_text():
         emit("H2C_G1_ISO", g1n + g1d + g1yn + g1yd, mont_words),
         "// Frobenius of Fp12: gamma_k = (1 + i)^(k (p - 1) / 6), k = 1..5",
         emit("PAIR_FROB", frobenius_constants()),
+        "// [1..8]G1, affine (Fp elements, 12 words each): x then y of [j]G1 at 24 (j - 1)",
+        emit_global("G1_TABLE", g1_table()),
         "}  // namespace bls",
         "}  // namespace b200",
         "",
