@@ -11,11 +11,13 @@
 //     trees is one dense array of independent pair additions, because every bucket's slots at every level are laid out by
 //     prefix sums of ceil(n_b / 2^r) (k_level_blocksums / k_level_scan / k_level_offsets): slot j of bucket b at level r+1 is the
 //     sum of slots 2j and 2j+1 of level r. No collisions exist by construction, nothing is queued or rescheduled.
-//   * k_affine_plan (one thread per sorted entry) writes, for every level, the source of each slot -- so the arithmetic kernels
-//     k_affine_pairs / k_affine_pairs_ws are plain list processors: lane = slot, perfectly regular, independent of the digit
-//     distribution. Both take their slots from PairSlots and do the arithmetic of a slot in pair_factor (pass 1) and
-//     pair_result (pass 2); they differ only in where the operands come from.
-//   * the shared inversion is PER THREAD: a thread walks M slots (M = level size / resident threads, ~150 at N = 2^20),
+//   * k_affine_plan (one thread per sorted entry) writes, for every level, the sources of each slot, into a pair list (slots
+//     with two operands) and a copy list (a bucket's last slot when its count at the level is odd) -- so the arithmetic kernels
+//     k_affine_pairs / k_affine_pairs_ws are plain list processors: lane = pair, perfectly regular, independent of the digit
+//     distribution. Both take their pairs from PairSlots and do the arithmetic of a pair in pair_factor (pass 1) and
+//     pair_result (pass 2); they differ only in where the operands come from. The copies run after the pairs, in the same
+//     launch (copy_singles), so no lane idles through the multiplications of a batch for a slot that has none.
+//   * the shared inversion is PER THREAD: a thread walks M pairs (M = pairs of the level / resident threads, ~150 at N = 2^20),
 //     multiplies their denominators into a running product (prefix products parked in a coalesced global scratch), inverts
 //     once (safegcd, field_inv.cuh) and unwinds: 1 + 5 multiplications per addition + inversion / M. Lanes never wait for
 //     each other: no block-wide scan, no barrier, every lane of a warp inverts at the same time.
@@ -31,7 +33,6 @@
 namespace b200 {
 
 constexpr int AFF_MAX_LEVELS = 8;
-constexpr uint32_t AFF_NONE = 0xFFFFFFFFu;
 
 // ------------------------------------------------------------------------------------------------ run bounds
 // head[b] = first sorted position of key b, tail[b] = one past its last (both pre-zeroed: empty buckets have length 0)
@@ -45,7 +46,10 @@ static __global__ void k_bucket_bounds(const uint32_t* __restrict__ keys, size_t
 }
 
 // ------------------------------------------------------------------------------------------------ level offsets
-// off[r * (nb + 1) + b] = sum_{b' < b} ceil(n_b' / 2^r) for r = 0..L; off[r * (nb + 1) + nb] = size of level r.
+// 2L + 1 rows of nb + 1 words; column nb holds the row's total.
+//   row r (r = 0..L):          off[r][b] = sum_{b' < b} ceil(n_b' / 2^r), the slots of level r before bucket b;
+//   row L + 1 + r (r < L):     sum_{b' < b} (ceil(n_b' / 2^r) mod 2), the single slots of level r (its copies) before bucket b.
+// A bucket's single slot is its last one, so level r's pairs before bucket b are off[r + 1][b] - off[L + 1 + r][b].
 // Three small kernels (block sums, scan of the block sums, offsets); a block covers SCAN_ITEMS buckets.
 constexpr int SCAN_THREADS = 256, SCAN_PER_THREAD = 4, SCAN_ITEMS = SCAN_THREADS * SCAN_PER_THREAD;
 
@@ -73,38 +77,50 @@ B200_DEV uint32_t block_exclusive_scan(uint32_t v, uint32_t& total, uint32_t* sm
 }
 
 B200_DEV uint32_t level_count(uint32_t n, int r) { return (n + (1u << r) - 1u) >> r; }
+// what row `row` of off counts for a bucket of n entries
+B200_DEV uint32_t offset_row_count(uint32_t n, int row, int L) { return row <= L ? level_count(n, row) : level_count(n, row - L - 1) & 1u; }
 
 static __global__ void __launch_bounds__(SCAN_THREADS) k_level_blocksums(const uint32_t* __restrict__ head, const uint32_t* __restrict__ tail,
-                                                                          uint32_t nb, int L, uint32_t nblk, uint32_t* blocksum /* [(L+1)][nblk] */) {
+                                                                          uint32_t nb, int L, uint32_t nblk, uint32_t* blocksum /* [2L+1][nblk] */) {
   __shared__ uint32_t sm[SCAN_THREADS / 32 + 1];
   const uint32_t b0 = blockIdx.x * SCAN_ITEMS + threadIdx.x * SCAN_PER_THREAD;
   uint32_t cnt[SCAN_PER_THREAD];
 #pragma unroll
   for (int k = 0; k < SCAN_PER_THREAD; k++) cnt[k] = (b0 + k < nb) ? tail[b0 + k] - head[b0 + k] : 0u;
-  for (int r = 0; r <= L; r++) {
+  for (int row = 0; row <= 2 * L; row++) {
     uint32_t s = 0;
 #pragma unroll
-    for (int k = 0; k < SCAN_PER_THREAD; k++) s += level_count(cnt[k], r);
+    for (int k = 0; k < SCAN_PER_THREAD; k++) s += offset_row_count(cnt[k], row, L);
     uint32_t tot;
     block_exclusive_scan(s, tot, sm);
-    if (threadIdx.x == 0) blocksum[(size_t)r * nblk + blockIdx.x] = tot;
+    if (threadIdx.x == 0) blocksum[(size_t)row * nblk + blockIdx.x] = tot;
   }
 }
 
-// one block: exclusive scan of the block sums of every level; also stores the level sizes at off[r][nb]
-static __global__ void __launch_bounds__(SCAN_THREADS) k_level_scan(uint32_t* blocksum, uint32_t nblk, int L, uint32_t nb, uint32_t* off) {
+// one block: exclusive scan of the block sums of every row; also stores the row totals at off[row][nb], and per pair level r
+// counts[2r] = its pairs, counts[2r + 1] = its copies (single slots)
+static __global__ void __launch_bounds__(SCAN_THREADS) k_level_scan(uint32_t* blocksum, uint32_t nblk, int L, uint32_t nb, uint32_t* off,
+                                                                    uint32_t* counts) {
   __shared__ uint32_t sm[SCAN_THREADS / 32 + 1];
-  for (int r = 0; r <= L; r++) {
+  const size_t stride = (size_t)nb + 1;
+  for (int row = 0; row <= 2 * L; row++) {
     uint32_t carry = 0;
     for (uint32_t base = 0; base < nblk; base += SCAN_THREADS) {
       const uint32_t i = base + threadIdx.x;
-      const uint32_t v = (i < nblk) ? blocksum[(size_t)r * nblk + i] : 0u;
+      const uint32_t v = (i < nblk) ? blocksum[(size_t)row * nblk + i] : 0u;
       uint32_t tot;
       const uint32_t ex = block_exclusive_scan(v, tot, sm);
-      if (i < nblk) blocksum[(size_t)r * nblk + i] = carry + ex;
+      if (i < nblk) blocksum[(size_t)row * nblk + i] = carry + ex;
       carry += tot;
     }
-    if (threadIdx.x == 0) off[(size_t)r * (nb + 1) + nb] = carry;
+    if (threadIdx.x == 0) off[(size_t)row * stride + nb] = carry;
+  }
+  if (threadIdx.x == 0) {
+    for (int r = 0; r < L; r++) {
+      const uint32_t copies = off[(size_t)(L + 1 + r) * stride + nb];
+      counts[2 * r] = off[(size_t)(r + 1) * stride + nb] - copies;
+      counts[2 * r + 1] = copies;
+    }
   }
 }
 
@@ -116,24 +132,29 @@ static __global__ void __launch_bounds__(SCAN_THREADS) k_level_offsets(const uin
   uint32_t cnt[SCAN_PER_THREAD];
 #pragma unroll
   for (int k = 0; k < SCAN_PER_THREAD; k++) cnt[k] = (b0 + k < nb) ? tail[b0 + k] - head[b0 + k] : 0u;
-  for (int r = 0; r <= L; r++) {
+  for (int row = 0; row <= 2 * L; row++) {
     uint32_t c[SCAN_PER_THREAD], s = 0;
 #pragma unroll
-    for (int k = 0; k < SCAN_PER_THREAD; k++) { c[k] = level_count(cnt[k], r); s += c[k]; }
+    for (int k = 0; k < SCAN_PER_THREAD; k++) { c[k] = offset_row_count(cnt[k], row, L); s += c[k]; }
     uint32_t tot;
-    uint32_t ex = block_exclusive_scan(s, tot, sm) + blocksum[(size_t)r * nblk + blockIdx.x];
+    uint32_t ex = block_exclusive_scan(s, tot, sm) + blocksum[(size_t)row * nblk + blockIdx.x];
 #pragma unroll
     for (int k = 0; k < SCAN_PER_THREAD; k++) {
-      if (b0 + k < nb) off[(size_t)r * (nb + 1) + b0 + k] = ex;
+      if (b0 + k < nb) off[(size_t)row * (nb + 1) + b0 + k] = ex;
       ex += c[k];
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------------ plan
+// The work of pair level r (level r -> r + 1) is two lists. The pair list holds the slots of level r + 1 with two operands, in slot
+// order, and the slot each fills; the copy list holds the single slots (the last slot of a bucket whose level-r count is odd), which
+// take no part in the shared inversion. Level-0 operands are point refs (index | sign << 31), the others slots of level r.
 struct AffinePlan {
-  uint2* plan0;                        // level 0 -> 1: (point ref | sign << 31, partner ref or AFF_NONE)
-  uint32_t* plan[AFF_MAX_LEVELS];      // level r -> r+1 (r >= 1): index of the left operand in level r | has-partner << 31
+  uint2* pairs0;                       // level 0: (left point ref, right point ref)
+  uint32_t* pairs[AFF_MAX_LEVELS];     // level r >= 1: index a of the left operand in level r; the right one is a + 1
+  uint32_t* pair_out[AFF_MAX_LEVELS];  // slot of level r + 1 that pair k fills
+  uint2* copies[AFF_MAX_LEVELS];       // (operand, slot of level r + 1 it is copied to)
   uint32_t* surv_keys;                 // survivors of level L: bucket key per slot (sorted), and the identity map as "point refs"
   uint32_t* surv_vals;
 };
@@ -153,9 +174,16 @@ static __global__ void k_affine_plan(const uint32_t* __restrict__ keys, const ui
     if (i & ((2u << r) - 1u)) break;
     const uint32_t p = off[(size_t)(r + 1) * stride + b] + (i >> (r + 1));
     const uint32_t s = i >> r;
-    const bool has2 = s + 1u < level_count(cnt, r);
-    if (r == 0) P.plan0[p] = make_uint2(vals[q], has2 ? vals[q + 1] : AFF_NONE);
-    else P.plan[r][p] = (off[(size_t)r * stride + b] + s) | (has2 ? 0x80000000u : 0u);
+    const uint32_t a = r == 0 ? vals[q] : off[(size_t)r * stride + b] + s;
+    const uint32_t singles_before = off[(size_t)(L + 1 + r) * stride + b];
+    if (s + 1u < level_count(cnt, r)) {
+      const uint32_t k = p - singles_before;     // the slots of level r + 1 before p, less the single ones
+      if (r == 0) P.pairs0[k] = make_uint2(a, vals[q + 1]);
+      else P.pairs[r][k] = a;
+      P.pair_out[r][k] = p;
+    } else {
+      P.copies[r][singles_before] = make_uint2(a, p);
+    }
   }
   if ((i & ((1u << L) - 1u)) == 0u) {
     const uint32_t ps = off[(size_t)L * stride + b] + (i >> L);
@@ -206,12 +234,11 @@ B200_DEV T scratch_load(const uint4* scratch, size_t threads, size_t tid, uint32
 // ------------------------------------------------------------------------------------------------ level 0 by arrival of the points
 // A host call moves its points over PCIe in P chunks. A level-0 pair only needs the chunks of its own operands, so the pair list is
 // partitioned (stable counting sort, P <= 8 classes) by the LAST chunk a pair touches: launch q of the pair kernel runs as soon as
-// chunk q has landed, and only the last launch waits for the whole transfer.
+// chunk q has landed, and only the last launch waits for the whole transfer. The level's copies run in the last launch.
 constexpr int PART_TILE = 1024, PART_THREADS = 256, PART_MAX = 8;
 
 B200_DEV uint32_t pair_chunk(const uint2 task, uint32_t n_points, uint32_t P) {
-  uint32_t idx = task.x & 0x7FFFFFFFu;
-  if (task.y != AFF_NONE) { const uint32_t j = task.y & 0x7FFFFFFFu; if (j > idx) idx = j; }
+  const uint32_t idx = max(task.x & 0x7FFFFFFFu, task.y & 0x7FFFFFFFu);
   uint32_t q = (uint32_t)(((unsigned long long)idx * P) / n_points);
   return q < P ? q : P - 1u;
 }
@@ -303,20 +330,29 @@ static __global__ void __launch_bounds__(PART_THREADS) k_part_scatter(const uint
 
 enum PairKind { PAIR_COPY1 = 0, PAIR_COPY2 = 1, PAIR_INF = 2, PAIR_ADD = 3, PAIR_DBL = 4 };
 
-// one slot's operands. FIRST: references into the caller's point array (sign in bit 31); else slots of the previous level.
+// The lists of one pair-kernel launch (AffinePlan): pairs (uint2 at level 0, else uint32), the slot each pair fills, and the copy list
+// of the level, or nullptr when another launch of the level runs it. The counts are on the device.
+struct PairLevel {
+  const void* pairs;
+  const uint32_t* out;
+  const uint32_t* npairs;
+  const uint2* copies;
+  const uint32_t* ncopies;
+};
+
+// one pair's operands. FIRST: references into the caller's point array (sign in bit 31); else slots of the previous level.
 struct PairTask {
-  uint32_t a, b;     // b == AFF_NONE: single operand
+  uint32_t a, b;
 };
 template <bool FIRST>
-B200_DEV PairTask load_task(const void* plan, size_t p) {
+B200_DEV PairTask load_task(const void* pairs, size_t k) {
   PairTask t;
   if constexpr (FIRST) {
-    const uint2 v = reinterpret_cast<const uint2*>(plan)[p];
+    const uint2 v = reinterpret_cast<const uint2*>(pairs)[k];
     t.a = v.x; t.b = v.y;
   } else {
-    const uint32_t v = reinterpret_cast<const uint32_t*>(plan)[p];
-    t.a = v & 0x7FFFFFFFu;
-    t.b = (v >> 31) ? t.a + 1u : AFF_NONE;
+    t.a = reinterpret_cast<const uint32_t*>(pairs)[k];
+    t.b = t.a + 1u;
   }
   return t;
 }
@@ -345,8 +381,7 @@ B200_DEV T load_y(const uint32_t* src, uint32_t ref, bool& zero) {
 
 // Classification shared by both passes. den is the factor this pair contributes to the batch product (ADD: x2 - x1, DBL: 2 y1).
 template <class T>
-B200_DEV int classify_pair(bool single, const T& x1, const T& y1, bool inf1, const T& x2, const T& y2, bool inf2, T& den) {
-  if (single) return PAIR_COPY1;
+B200_DEV int classify_pair(const T& x1, const T& y1, bool inf1, const T& x2, const T& y2, bool inf2, T& den) {
   if (inf1) return PAIR_COPY2;
   if (inf2) return PAIR_COPY1;
   den = x2 - x1;
@@ -357,29 +392,28 @@ B200_DEV int classify_pair(bool single, const T& x1, const T& y1, bool inf1, con
 }
 
 // The slot arithmetic of both pair kernels, which differ only in where the operands come from.
-// Pass 1 of slot (a, b): multiplies its factor, if it has one, into the running product, from the abscissae as loaded.
+// Pass 1 of pair (a, b): multiplies its factor, if it has one, into the running product, from the abscissae as loaded.
 template <class T, bool FIRST>
 B200_DEV void pair_factor(const uint32_t* src, uint32_t a, uint32_t b, const T& x1, const T& x2, T& run) {
-  const bool single = b == AFF_NONE;
   T den = x2 - x1;
-  bool contributes = !single;
-  if (!single && (den.is_zero() || x1.is_zero() || x2.is_zero())) {
+  bool contributes = true;
+  if (den.is_zero() || x1.is_zero() || x2.is_zero()) {
     // rare: equal abscissae (doubling or cancellation) or a possible infinity operand -- needs the ordinates
     bool z1, z2;
     const T y1 = load_y<T, FIRST>(src, a, z1), y2 = load_y<T, FIRST>(src, b, z2);
-    const int kind = classify_pair(false, x1, y1, z1 && x1.is_zero(), x2, y2, z2 && x2.is_zero(), den);
+    const int kind = classify_pair(x1, y1, z1 && x1.is_zero(), x2, y2, z2 && x2.is_zero(), den);
     contributes = kind >= PAIR_ADD;
   }
   if (contributes) run = run.mul_u(den);
 }
 
-// Pass 2 of slot j: R = P1 + P2 from the decoded operands and their y = 0 flags (P2 unused when single). inv is the inverse of
-// the running product up to slot j and moves past it; prefix() returns the running product before slot j, and is called only
-// for an addition or a doubling of a slot j > 0.
+// Pass 2 of pair j: R = P1 + P2 from the decoded operands and their y = 0 flags. inv is the inverse of the running product up to
+// pair j and moves past it; prefix() returns the running product before pair j, and is called only for an addition or a doubling
+// of a pair j > 0.
 template <class T, class Prefix>
-B200_DEV Aff<T> pair_result(const Aff<T>& P1, bool z1, const Aff<T>& P2, bool z2, bool single, uint32_t j, T& inv, Prefix prefix) {
+B200_DEV Aff<T> pair_result(const Aff<T>& P1, bool z1, const Aff<T>& P2, bool z2, uint32_t j, T& inv, Prefix prefix) {
   T den;
-  const int kind = classify_pair(single, P1.x, P1.y, z1 && P1.x.is_zero(), P2.x, P2.y, z2 && P2.x.is_zero(), den);
+  const int kind = classify_pair(P1.x, P1.y, z1 && P1.x.is_zero(), P2.x, P2.y, z2 && P2.x.is_zero(), den);
   Aff<T> R;
   if (kind < PAIR_ADD) {
     if (kind == PAIR_COPY1) R = P1;
@@ -419,13 +453,13 @@ B200_DEV void prefetch_point(const uint32_t* src, uint32_t ref) {
   prefetch_span(src + (size_t)idx * (2 * T::WORDS), 2 * T::WORDS * 4);
 }
 
-// Slots, and rows of the prefix-product scratch, per slot-owning thread for a level of `slots` slots.
-__host__ __device__ __forceinline__ size_t pair_rows(size_t slots, size_t threads) { return (slots + threads - 1) / threads; }
+// Pairs, and rows of the prefix-product scratch, per slot-owning thread for a level of `pairs` pairs.
+__host__ __device__ __forceinline__ size_t pair_rows(size_t pairs, size_t threads) { return (pairs + threads - 1) / threads; }
 
-// The slot schedule of a pair-kernel launch. The `threads` slot-owning threads of the grid split the slots evenly: a warp owns a
-// contiguous range of 32 M slots and lane l takes slots l, l + 32, ... of it (coalesced plans, outputs and level >= 1 operands).
-// perm / range (level 0 of a host call whose points arrive in pieces): the launch handles the slots perm[range[0] .. range[1]),
-// i.e. the pairs whose operands all lie in the pieces that have arrived; otherwise slots 0 .. *total_ptr in order.
+// The pair schedule of a pair-kernel launch. The `threads` slot-owning threads of the grid split the pair list evenly: a warp owns a
+// contiguous range of 32 M pairs and lane l takes pairs l, l + 32, ... of it (coalesced lists, outputs and level >= 1 operands).
+// perm / range (level 0 of a host call whose points arrive in pieces): the launch handles the pairs perm[range[0] .. range[1]),
+// i.e. the pairs whose operands all lie in the pieces that have arrived; otherwise pairs 0 .. *total_ptr in order.
 // tid: index of a thread among the slot-owning threads.
 struct PairSlots {
   const uint32_t* perm;
@@ -438,7 +472,7 @@ struct PairSlots {
     M = (uint32_t)pair_rows(total, threads);
   }
   B200_DEV size_t first(size_t tid) const { return (tid & ~(size_t)31) * M + (tid & 31u); }
-  // slots of the thread: first + 32 j for j < count
+  // pairs of the thread: first + 32 j for j < count
   B200_DEV uint32_t count(size_t tid) const {
     const size_t f = first(tid);
     if (f >= total) return 0u;
@@ -451,34 +485,54 @@ struct PairSlots {
   }
 };
 
-// dst[p] = src[a_p] (+ src[b_p]) for the slots p of PairSlots. Persistent: every thread owns slots.
+// The copy list of a launch, after its pairs: dst[out] = src[operand], at level 0 with the sign applied (infinity stays (0, 0)).
+// Strided over all slot-owning threads, so every lane of a warp copies at the same time.
+template <class T, bool FIRST>
+B200_DEV void copy_singles(const PairLevel& lv, const uint32_t* src, uint32_t* dst, size_t threads, size_t tid) {
+  if (!lv.copies) return;
+  const uint32_t n = *lv.ncopies;
+#pragma unroll 1
+  for (size_t k = tid; k < n; k += threads) {
+    const uint2 c = lv.copies[k];
+    Aff<T> P;
+    bool z;
+    P.x = load_x<T, FIRST>(src, c.x);
+    P.y = load_y<T, FIRST>(src, c.x, z);
+    store_affine(dst, c.y, P);
+  }
+}
+
+// dst[out_k] = src[a_k] + src[b_k] for the pairs k of PairSlots, then the copies. Persistent: every thread owns pairs.
 template <class T, bool FIRST>
 __global__ void __launch_bounds__(B200_AFF_THREADS, (T::WORDS <= 12) ? B200_AFF_MIN_BLOCKS : 1)
-k_affine_pairs(const void* __restrict__ plan, const uint32_t* __restrict__ total_ptr, const uint32_t* src, uint32_t* dst, uint4* scratch,
+k_affine_pairs(const PairLevel lv, const uint32_t* src, uint32_t* dst, uint4* scratch,
                const uint32_t* __restrict__ perm = nullptr, const uint32_t* __restrict__ range = nullptr) {
   const size_t threads = (size_t)gridDim.x * blockDim.x;
   const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const PairSlots S(total_ptr, perm, range, threads);
+  const PairSlots S(lv.npairs, perm, range, threads);
   const unsigned lane = threadIdx.x & 31u;
-  if (S.count(tid - lane) == 0) return;      // no slot for this warp
+  if (S.count(tid - lane) == 0) {      // no pair for this warp
+    copy_singles<T, FIRST>(lv, src, dst, threads, tid);
+    return;
+  }
   const uint32_t cnt = S.count(tid);
   // ---- pass 1: running product of the denominators; prefix products to the scratch
   T run = T::one();
   {
-    PairTask t_next = cnt ? load_task<FIRST>(plan, S.slot(tid, 0)) : PairTask{0u, AFF_NONE};
+    PairTask t_next = cnt ? load_task<FIRST>(lv.pairs, S.slot(tid, 0)) : PairTask{0u, 0u};
     T x1n = T::zero(), x2n = T::zero();
     if (cnt) {
       x1n = load_x<T, FIRST>(src, t_next.a);
-      if (t_next.b != AFF_NONE) x2n = load_x<T, FIRST>(src, t_next.b);
+      x2n = load_x<T, FIRST>(src, t_next.b);
     }
 #pragma unroll 1
     for (uint32_t j = 0; j < cnt; j++) {
       const PairTask t = t_next;
       const T x1 = x1n, x2 = x2n;
       if (j + 1 < cnt) {
-        t_next = load_task<FIRST>(plan, S.slot(tid, j + 1));
+        t_next = load_task<FIRST>(lv.pairs, S.slot(tid, j + 1));
         x1n = load_x<T, FIRST>(src, t_next.a);
-        if (t_next.b != AFF_NONE) x2n = load_x<T, FIRST>(src, t_next.b);
+        x2n = load_x<T, FIRST>(src, t_next.b);
       }
       pair_factor<T, FIRST>(src, t.a, t.b, x1, x2, run);
       scratch_store(scratch, threads, tid, j, run);
@@ -486,39 +540,37 @@ k_affine_pairs(const void* __restrict__ plan, const uint32_t* __restrict__ total
   }
   // ---- the shared inversion of this thread's batch
   T inv = fe_inverse(run);
-  // ---- pass 2: unwind, last slot first. The operands of slot j - 1 (found through its plan entry) and the prefix product it
-  // will need are pulled into L2 while slot j is being computed: the dependent plan -> point gather then costs an L2 hit.
-  size_t p_prev = cnt ? S.slot(tid, cnt - 1) : 0;
-  PairTask t_prev = cnt ? load_task<FIRST>(plan, p_prev) : PairTask{0u, AFF_NONE};
+  // ---- pass 2: unwind, last pair first. The operands of pair j - 1 (found through its list entry) and the prefix product it
+  // will need are pulled into L2 while pair j is being computed: the dependent list -> point gather then costs an L2 hit.
+  size_t k_prev = cnt ? S.slot(tid, cnt - 1) : 0;
+  PairTask t_prev = cnt ? load_task<FIRST>(lv.pairs, k_prev) : PairTask{0u, 0u};
+  uint32_t out_prev = cnt ? lv.out[k_prev] : 0u;
 #pragma unroll 1
   for (uint32_t jj = cnt; jj > 0; jj--) {
     const uint32_t j = jj - 1;
-    const size_t p = p_prev;
+    const uint32_t out = out_prev;
     const PairTask t = t_prev;
     if (j > 0) {
-      p_prev = S.slot(tid, j - 1);
-      t_prev = load_task<FIRST>(plan, p_prev);
+      k_prev = S.slot(tid, j - 1);
+      t_prev = load_task<FIRST>(lv.pairs, k_prev);
+      out_prev = lv.out[k_prev];
       prefetch_point<T, FIRST>(src, t_prev.a);
-      if (t_prev.b != AFF_NONE) prefetch_point<T, FIRST>(src, t_prev.b);
+      prefetch_point<T, FIRST>(src, t_prev.b);
       if (j > 1) {
         constexpr int V = T::WORDS / 4;
 #pragma unroll
         for (int k = 0; k < V; k++) prefetch_l2(scratch + ((size_t)(j - 2) * V + k) * threads + tid);
       }
     }
-    const bool single = t.b == AFF_NONE;
     Aff<T> P1, P2;
-    bool z1 = false, z2 = false;
+    bool z1, z2;
     P1.x = load_x<T, FIRST>(src, t.a);
     P1.y = load_y<T, FIRST>(src, t.a, z1);
-    if (!single) {
-      P2.x = load_x<T, FIRST>(src, t.b);
-      P2.y = load_y<T, FIRST>(src, t.b, z2);
-    } else {
-      P2.x = T::zero(); P2.y = T::zero();
-    }
-    store_affine(dst, p, pair_result(P1, z1, P2, z2, single, j, inv, [&] { return scratch_load<T>(scratch, threads, tid, j - 1); }));
+    P2.x = load_x<T, FIRST>(src, t.b);
+    P2.y = load_y<T, FIRST>(src, t.b, z2);
+    store_affine(dst, out, pair_result(P1, z1, P2, z2, j, inv, [&] { return scratch_load<T>(scratch, threads, tid, j - 1); }));
   }
+  copy_singles<T, FIRST>(lv, src, dst, threads, tid);
 }
 
 // ------------------------------------------------------------------------------------------------ warp-specialised pair kernel
@@ -587,13 +639,12 @@ B200_DEV T ring_load(const uint4* ring, int row, unsigned lane) {
 
 template <class T, bool FIRST>
 __global__ void __launch_bounds__(AFF_WS_THREADS, 1)
-k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ total_ptr, const uint32_t* src, uint32_t* dst, uint4* scratch,
-                  const uint32_t* __restrict__ perm = nullptr, const uint32_t* __restrict__ range = nullptr) {
+k_affine_pairs_ws(const PairLevel lv, const uint32_t* src, uint32_t* dst, uint4* scratch, const uint32_t* __restrict__ perm = nullptr, const uint32_t* __restrict__ range = nullptr) {
   using RG = AffRing<T>;
   constexpr int V = RG::V, NC = AFF_WS_CONSUMERS, S1 = RG::S1, S2 = RG::S2;
   extern __shared__ __align__(16) unsigned char aff_ring_raw[];
   __shared__ uint64_t full1[NC][S1], empty1[NC][S1], full2[NC][S2], empty2[NC][S2], drained[NC];
-  __shared__ uint32_t s_task[NC][S1][3][32];          // (a, b, output slot) of each lane's slot in a stage
+  __shared__ uint32_t s_task[NC][S1][3][32];          // (a, b, output slot) of each lane's pair in a stage
   const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   if (threadIdx.x == 0) {
     for (int w = 0; w < NC; w++) {
@@ -603,9 +654,9 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
     }
   }
   __syncthreads();
-  // the slots are those of the consumer threads only
+  // the pairs and copies are those of the consumer threads only
   const size_t threads = (size_t)gridDim.x * NC * 32;
-  const PairSlots S(total_ptr, perm, range, threads);
+  const PairSlots S(lv.npairs, perm, range, threads);
   uint4* const ring_base = reinterpret_cast<uint4*>(aff_ring_raw);
 
   if (warp == NC) {
@@ -614,28 +665,29 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
 #pragma unroll
     for (int w = 0; w < NC; w++) {
       const size_t tid = ((size_t)blockIdx.x * NC + w) * 32 + lane;
-      n[w] = S.count(tid - lane);                 // iterations of warp w (lane 0 has the most slots)
+      n[w] = S.count(tid - lane);                 // iterations of warp w (lane 0 has the most pairs)
       cnt[w] = S.count(tid);
     }
     auto tid_of = [&](int w) { return ((size_t)blockIdx.x * NC + w) * 32 + lane; };
     auto src_of = [&](uint32_t ref) { return src + (size_t)(FIRST ? (ref & 0x7FFFFFFFu) : ref) * (2 * T::WORDS); };
-    // the plan entries of the next round are loaded while this round's copies are issued
+    // the list entries of the next round are loaded while this round's copies are issued; pass 2 also needs the output slot
     uint32_t ta[NC], tb[NC], tp[NC];
-    auto fetch_task = [&](int w, uint32_t j) {
-      const size_t p = S.slot(tid_of(w), j);
-      const PairTask t = load_task<FIRST>(plan, p);
-      ta[w] = t.a; tb[w] = t.b; tp[w] = (uint32_t)p;
+    auto fetch_task = [&](int w, uint32_t j, bool with_out) {
+      const size_t k = S.slot(tid_of(w), j);
+      const PairTask t = load_task<FIRST>(lv.pairs, k);
+      ta[w] = t.a; tb[w] = t.b;
+      if (with_out) tp[w] = lv.out[k];
     };
     // ---- pass 1: x1, x2
 #pragma unroll
-    for (int w = 0; w < NC; w++) if (cnt[w]) fetch_task(w, 0);
+    for (int w = 0; w < NC; w++) if (cnt[w]) fetch_task(w, 0, false);
 #pragma unroll 1
     for (uint32_t j = 0; j < n[0]; j++) {
       uint32_t ca[NC], cb[NC];
 #pragma unroll
       for (int w = 0; w < NC; w++) { ca[w] = ta[w]; cb[w] = tb[w]; }
 #pragma unroll
-      for (int w = 0; w < NC; w++) if (j + 1 < cnt[w]) fetch_task(w, j + 1);
+      for (int w = 0; w < NC; w++) if (j + 1 < cnt[w]) fetch_task(w, j + 1, false);
 #pragma unroll
       for (int w = 0; w < NC; w++) {
         if (j >= n[w]) continue;
@@ -646,22 +698,22 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
           s_task[w][s][0][lane] = ca[w];
           s_task[w][s][1][lane] = cb[w];
           ring_fetch<T>(ring, s * 2 * V, lane, src_of(ca[w]));
-          if (cb[w] != AFF_NONE) ring_fetch<T>(ring, s * 2 * V + V, lane, src_of(cb[w]));
+          ring_fetch<T>(ring, s * 2 * V + V, lane, src_of(cb[w]));
         }
         cp_async_arrive(&full1[w][s]);
         mbar_arrive(&full1[w][s]);
       }
     }
-    // ---- pass 2, last slot first: P1, P2, prefix product of the slot before
+    // ---- pass 2, last pair first: P1, P2, prefix product of the pair before
 #pragma unroll
-    for (int w = 0; w < NC; w++) if (n[w] && n[w] - 1 < cnt[w]) fetch_task(w, n[w] - 1);
+    for (int w = 0; w < NC; w++) if (n[w] && n[w] - 1 < cnt[w]) fetch_task(w, n[w] - 1, true);
 #pragma unroll 1
     for (uint32_t jj = 0; jj < n[0]; jj++) {
       uint32_t ca[NC], cb[NC], cp[NC];
 #pragma unroll
       for (int w = 0; w < NC; w++) { ca[w] = ta[w]; cb[w] = tb[w]; cp[w] = tp[w]; }
 #pragma unroll
-      for (int w = 0; w < NC; w++) if (jj + 1 < n[w] && n[w] - 2 - jj < cnt[w]) fetch_task(w, n[w] - 2 - jj);
+      for (int w = 0; w < NC; w++) if (jj + 1 < n[w] && n[w] - 2 - jj < cnt[w]) fetch_task(w, n[w] - 2 - jj, true);
 #pragma unroll
       for (int w = 0; w < NC; w++) {
         if (jj >= n[w]) continue;
@@ -677,10 +729,8 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
           const int row = s * 5 * V;
           ring_fetch<T>(ring, row, lane, src_of(ca[w]));
           ring_fetch<T>(ring, row + V, lane, src_of(ca[w]) + T::WORDS);
-          if (cb[w] != AFF_NONE) {
-            ring_fetch<T>(ring, row + 2 * V, lane, src_of(cb[w]));
-            ring_fetch<T>(ring, row + 3 * V, lane, src_of(cb[w]) + T::WORDS);
-          }
+          ring_fetch<T>(ring, row + 2 * V, lane, src_of(cb[w]));
+          ring_fetch<T>(ring, row + 3 * V, lane, src_of(cb[w]) + T::WORDS);
           if (j > 0) {
 #pragma unroll
             for (int k = 0; k < V; k++)
@@ -698,7 +748,10 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
   // ================= consumers
   const size_t tid = ((size_t)blockIdx.x * NC + warp) * 32 + lane;
   const uint32_t n = S.count(tid - lane), cnt = S.count(tid);
-  if (n == 0) return;
+  if (n == 0) {
+    copy_singles<T, FIRST>(lv, src, dst, threads, tid);
+    return;
+  }
   const uint4* ring = ring_base + (size_t)warp * RG::ROWS * 32;
   // ---- pass 1: running product of the denominators; prefix products to the scratch
   T run = T::one();
@@ -716,7 +769,7 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
   mbar_arrive(&drained[warp]);      // release: the producer's pass-2 copies of the prefix products come after these stores
   // ---- the shared inversion of this thread's batch
   T inv = fe_inverse(run);
-  // ---- pass 2: unwind, last slot first
+  // ---- pass 2: unwind, last pair first
 #pragma unroll 1
   for (uint32_t jj = 0; jj < n; jj++) {
     const uint32_t j = n - 1 - jj;
@@ -724,20 +777,20 @@ k_affine_pairs_ws(const void* __restrict__ plan, const uint32_t* __restrict__ to
     mbar_wait(&full2[warp][s], (jj / S2) & 1u);
     const int row = s * 5 * V;
     const uint32_t a = s_task[warp][s][0][lane], b = s_task[warp][s][1][lane], p = s_task[warp][s][2][lane];
-    const bool single = b == AFF_NONE;
     Aff<T> P1, P2;
     P1.x = ring_load<T>(ring, row, lane);
     P1.y = ring_load<T>(ring, row + V, lane);
-    P2.x = single ? T::zero() : ring_load<T>(ring, row + 2 * V, lane);
-    P2.y = single ? T::zero() : ring_load<T>(ring, row + 3 * V, lane);
+    P2.x = ring_load<T>(ring, row + 2 * V, lane);
+    P2.y = ring_load<T>(ring, row + 3 * V, lane);
     const T pre = ring_load<T>(ring, row + 4 * V, lane);
     mbar_arrive(&empty2[warp][s]);
     if (j >= cnt) continue;
-    bool z1, z2 = false;
+    bool z1, z2;
     decode_y<T, FIRST>(P1.y, a, z1);
-    if (!single) decode_y<T, FIRST>(P2.y, b, z2);
-    store_affine(dst, p, pair_result(P1, z1, P2, z2, single, j, inv, [&] { return pre; }));
+    decode_y<T, FIRST>(P2.y, b, z2);
+    store_affine(dst, p, pair_result(P1, z1, P2, z2, j, inv, [&] { return pre; }));
   }
+  copy_singles<T, FIRST>(lv, src, dst, threads, tid);
 }
 
 // The pair kernel of a level: the warp-specialised one where its ring fits in shared memory, k_affine_pairs otherwise.
@@ -745,7 +798,7 @@ template <class T>
 struct PairKernel {
   static constexpr bool WS = AffRing<T>::USED;
   static constexpr int THREADS = WS ? AFF_WS_THREADS : B200_AFF_THREADS;                 // per block
-  static constexpr int SLOT_THREADS = WS ? 32 * AFF_WS_CONSUMERS : B200_AFF_THREADS;     // per block, that own slots
+  static constexpr int SLOT_THREADS = WS ? 32 * AFF_WS_CONSUMERS : B200_AFF_THREADS;     // per block, that own pairs and copies
   static constexpr int SMEM = WS ? (int)AffRing<T>::BYTES : 0;                           // dynamic shared memory per block
   template <bool FIRST>
   static auto entry() {
@@ -770,10 +823,10 @@ cudaError_t affine_pairs_blocks_per_sm(int* bps) {
 }
 
 template <class T, bool FIRST>
-void launch_affine_pairs(unsigned grid, cudaStream_t s, const void* plan, const uint32_t* total_ptr, const uint32_t* src, uint32_t* dst, uint4* scratch,
+void launch_affine_pairs(unsigned grid, cudaStream_t s, const PairLevel& lv, const uint32_t* src, uint32_t* dst, uint4* scratch,
                          const uint32_t* perm = nullptr, const uint32_t* range = nullptr) {
   using K = PairKernel<T>;
-  K::template entry<FIRST>()<<<grid, K::THREADS, K::SMEM, s>>>(plan, total_ptr, src, dst, scratch, perm, range);
+  K::template entry<FIRST>()<<<grid, K::THREADS, K::SMEM, s>>>(lv, src, dst, scratch, perm, range);
 }
 
 }  // namespace b200

@@ -179,9 +179,11 @@ struct Engine {
   static constexpr int MAX_INPUT_CHUNKS = 8;
   cudaEvent_t ev_chunk[MAX_INPUT_CHUNKS];
   DeviceBuffer d_scalars, d_points, keys_a, keys_b, vals_a, vals_b, cub_tmp, buckets, part_pts[2], part_keys[2], red_a, red_b, red_planes, bounds;
-  // batched-affine levels: run bounds, level offsets, per-level plans, two work arrays (odd / even levels), the prefix-product
-  // scratch of the per-thread batch inversions and the survivor list handed to the XYZZ slice kernel
-  DeviceBuffer aff_head, aff_tail, aff_off, aff_blocksum, aff_plan[AFF_MAX_LEVELS], aff_work[2], aff_scratch, keys_s, vals_s, part_counts, part_starts, part_perm;
+  // batched-affine levels: run bounds, level offsets (and each level's pair and copy counts), per-level pair lists with the slot
+  // each pair fills and copy lists, two work arrays (odd / even levels), the prefix-product scratch of the per-thread batch
+  // inversions and the survivor list handed to the XYZZ slice kernel
+  DeviceBuffer aff_head, aff_tail, aff_off, aff_blocksum, aff_plan[AFF_MAX_LEVELS], aff_out[AFF_MAX_LEVELS], aff_copy[AFF_MAX_LEVELS], aff_work[2],
+      aff_scratch, keys_s, vals_s, part_counts, part_starts, part_perm;
   // EIP-4844 proofs (kzg_kernels.cuh): the blobs as Fr residues, the opening points and y = p(z)
   DeviceBuffer kzg_poly, kzg_args;
   // EIP-7594 cells and proofs (peerdas_kernels.cuh): natural-order coefficients, cells 64-127, the bank MSMs' results, the proofs
@@ -576,10 +578,13 @@ void affine_levels(Engine& E, const MsmSizes& z, int AL, size_t entries, size_t 
   const uint32_t nblk = (nb + SCAN_ITEMS - 1) / SCAN_ITEMS;
   const size_t off_stride = (size_t)nb + 1;
   E.aff_head.ensure((size_t)nb * 4); E.aff_tail.ensure((size_t)nb * 4);
-  E.aff_off.ensure((size_t)(AL + 1) * off_stride * 4);
-  E.aff_blocksum.ensure((size_t)(AL + 1) * nblk * 4);
-  E.aff_plan[0].ensure(level_cap(1) * 8);
-  for (int r = 1; r < AL; r++) E.aff_plan[r].ensure(level_cap(r + 1) * 4);
+  E.aff_off.ensure(((size_t)(2 * AL + 1) * off_stride + 2 * AL) * 4);   // the offset rows, then the pair / copy counts of each level
+  E.aff_blocksum.ensure((size_t)(2 * AL + 1) * nblk * 4);
+  for (int r = 0; r < AL; r++) {
+    E.aff_plan[r].ensure(level_cap(r + 1) * (r == 0 ? 8 : 4));
+    E.aff_out[r].ensure(level_cap(r + 1) * 4);
+    E.aff_copy[r].ensure((size_t)nb * 8);                       // at most one single slot per bucket
+  }
   E.aff_work[1].ensure(level_cap(1) * AFF_BYTES);               // odd levels
   if (AL >= 2) E.aff_work[0].ensure(level_cap(2) * AFF_BYTES);  // even levels
   E.keys_s.ensure(acc_entries * 4);
@@ -595,51 +600,59 @@ void affine_levels(Engine& E, const MsmSizes& z, int AL, size_t entries, size_t 
   }
   const unsigned aff_grid = (unsigned)(E.sm_count * bps);
   const size_t aff_threads = (size_t)aff_grid * PairKernel<T>::SLOT_THREADS;
-  E.aff_scratch.ensure(pair_rows(level_cap(1), aff_threads) * aff_threads * (size_t)T::WORDS * 4);
+  // level 0 has the most pairs (sum_b floor(n_b / 2) <= entries / 2), and no level more than the one before
+  E.aff_scratch.ensure(pair_rows(entries / 2, aff_threads) * aff_threads * (size_t)T::WORDS * 4);
   uint32_t* head = (uint32_t*)E.aff_head.ptr;
   uint32_t* tail = (uint32_t*)E.aff_tail.ptr;
   uint32_t* off = (uint32_t*)E.aff_off.ptr;
+  uint32_t* counts = off + (size_t)(2 * AL + 1) * off_stride;
   B200_CUDA_CHECK(cudaMemsetAsync(head, 0, (size_t)nb * 4, s));
   B200_CUDA_CHECK(cudaMemsetAsync(tail, 0, (size_t)nb * 4, s));
   B200_CUDA_CHECK(cudaMemsetAsync(E.keys_s.ptr, 0xFF, acc_entries * 4, s));   // KEY_NONE: the unused tail sorts last, like zero digits
   const unsigned eb = (unsigned)((entries + 255) / 256);
   k_bucket_bounds<<<eb, 256, 0, s>>>(keys, entries, z.no_key, head, tail);
   k_level_blocksums<<<nblk, SCAN_THREADS, 0, s>>>(head, tail, nb, AL, nblk, (uint32_t*)E.aff_blocksum.ptr);
-  k_level_scan<<<1, SCAN_THREADS, 0, s>>>((uint32_t*)E.aff_blocksum.ptr, nblk, AL, nb, off);
+  k_level_scan<<<1, SCAN_THREADS, 0, s>>>((uint32_t*)E.aff_blocksum.ptr, nblk, AL, nb, off, counts);
   k_level_offsets<<<nblk, SCAN_THREADS, 0, s>>>(head, tail, nb, AL, nblk, (const uint32_t*)E.aff_blocksum.ptr, off);
   AffinePlan aplan;
-  aplan.plan0 = (uint2*)E.aff_plan[0].ptr;
-  for (int r = 0; r < AFF_MAX_LEVELS; r++) aplan.plan[r] = (r >= 1 && r < AL) ? (uint32_t*)E.aff_plan[r].ptr : nullptr;
+  aplan.pairs0 = (uint2*)E.aff_plan[0].ptr;
+  for (int r = 0; r < AFF_MAX_LEVELS; r++) {
+    aplan.pairs[r] = (r >= 1 && r < AL) ? (uint32_t*)E.aff_plan[r].ptr : nullptr;
+    aplan.pair_out[r] = r < AL ? (uint32_t*)E.aff_out[r].ptr : nullptr;
+    aplan.copies[r] = r < AL ? (uint2*)E.aff_copy[r].ptr : nullptr;
+  }
   aplan.surv_keys = (uint32_t*)E.keys_s.ptr;
   aplan.surv_vals = (uint32_t*)E.vals_s.ptr;
   k_affine_plan<<<eb, 256, 0, s>>>(keys, vals, entries, z.no_key, head, tail, off, nb, AL, aplan);
   const bool split0 = PC > 1;
   if (!split0) wait_points(s, PC, pc, points_ready);
   for (int r = 0; r < AL; r++) {
-    const uint32_t* total_ptr = off + (size_t)(r + 1) * off_stride + nb;      // size of level r + 1
+    const PairLevel lv{E.aff_plan[r].ptr, (const uint32_t*)E.aff_out[r].ptr, counts + 2 * r, (const uint2*)E.aff_copy[r].ptr, counts + 2 * r + 1};
     uint32_t* dst = (uint32_t*)E.aff_work[(r + 1) & 1].ptr;
     if (r == 0 && split0) {
       // level 0 by arrival of the point pieces: stable partition of the pair list by the last piece a pair touches, one launch
-      // per piece behind that piece's event (k_part_* in msm_affine.cuh)
+      // per piece behind that piece's event (k_part_* in msm_affine.cuh); the copies run in the last one
       const uint32_t Pq = (uint32_t)PC;
       const uint32_t nblk_p = (uint32_t)((level_cap(1) + PART_TILE - 1) / PART_TILE);
       E.part_counts.ensure((size_t)Pq * nblk_p * 4);
       E.part_starts.ensure((size_t)(Pq + 1) * 4);
       E.part_perm.ensure(level_cap(1) * 4);
-      k_part_count<<<nblk_p, PART_THREADS, 0, s>>>((const uint2*)E.aff_plan[0].ptr, total_ptr, (uint32_t)nper, Pq, nblk_p, (uint32_t*)E.part_counts.ptr);
+      k_part_count<<<nblk_p, PART_THREADS, 0, s>>>((const uint2*)E.aff_plan[0].ptr, lv.npairs, (uint32_t)nper, Pq, nblk_p, (uint32_t*)E.part_counts.ptr);
       k_part_scan<<<1, SCAN_THREADS, 0, s>>>((uint32_t*)E.part_counts.ptr, Pq, nblk_p, (uint32_t*)E.part_starts.ptr);
-      k_part_scatter<<<nblk_p, PART_THREADS, 0, s>>>((const uint2*)E.aff_plan[0].ptr, total_ptr, (uint32_t)nper, Pq, nblk_p,
+      k_part_scatter<<<nblk_p, PART_THREADS, 0, s>>>((const uint2*)E.aff_plan[0].ptr, lv.npairs, (uint32_t)nper, Pq, nblk_p,
                                                       (const uint32_t*)E.part_counts.ptr, (uint32_t*)E.part_perm.ptr);
       for (int q = 0; q < PC; q++) {
         wait_piece(s, *pc, q);
-        launch_affine_pairs<T, true>(aff_grid, s, E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr,
+        PairLevel piece = lv;
+        if (q + 1 < PC) piece.copies = nullptr;
+        launch_affine_pairs<T, true>(aff_grid, s, piece, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr,
                                      (const uint32_t*)E.part_perm.ptr, (const uint32_t*)E.part_starts.ptr + q);
       }
       launches += 3 + PC - 1;
     } else if (r == 0)
-      launch_affine_pairs<T, true>(aff_grid, s, E.aff_plan[0].ptr, total_ptr, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr);
+      launch_affine_pairs<T, true>(aff_grid, s, lv, (const uint32_t*)pts, dst, (uint4*)E.aff_scratch.ptr);
     else
-      launch_affine_pairs<T, false>(aff_grid, s, E.aff_plan[r].ptr, total_ptr, (const uint32_t*)E.aff_work[r & 1].ptr, dst, (uint4*)E.aff_scratch.ptr);
+      launch_affine_pairs<T, false>(aff_grid, s, lv, (const uint32_t*)E.aff_work[r & 1].ptr, dst, (uint4*)E.aff_scratch.ptr);
   }
   keys = (const uint32_t*)E.keys_s.ptr;
   vals = (const uint32_t*)E.vals_s.ptr;

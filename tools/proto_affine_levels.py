@@ -1,12 +1,15 @@
 """CPU model of the batched-affine level schedule of constantine_b200/csrc/msm_affine.cuh, statement for statement:
-k_bucket_bounds -> level offsets -> k_affine_plan -> k_affine_pairs (per-thread batches with ONE shared inversion each,
-prefix products, special cases) -> survivor list. Exact arithmetic (oracle/pyref.py), tiny sizes.
+k_bucket_bounds -> level offsets -> k_affine_plan (a pair list and a copy list per level) -> k_affine_pairs (per-thread batches
+of pairs with ONE shared inversion each, prefix products, special cases, then the copies) -> survivor list. Exact arithmetic
+(oracle/pyref.py), tiny sizes.
 
 Checks, for random and adversarial runs (single entries, P + P, P - P, infinity operands, one giant run):
-  * every slot of every level is written exactly once;
+  * every slot of every level is written exactly once, by a pair or by a copy;
   * per bucket, the sum of its survivors equals the sum of its entries;
   * the shared inversion is used once per thread and level, never on a zero.
-Run: python tools/proto_affine_levels.py      (also imported by tests/test_host_logic.py)"""
+Run: python tools/proto_affine_levels.py      (also imported by tests/test_host_logic.py)
+     python tools/proto_affine_levels.py --bench-table [--logn 20 --c 16 --levels 3]
+         slots and single (copy) slots of each pair level for bench.py's scalars (seed 0xC770003), BLS12-381 G1"""
 import os
 import random
 import sys
@@ -15,9 +18,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from constantine_b200.curves import CURVES  # noqa: E402
 from oracle import pyref  # noqa: E402
-
-NONE = 0xFFFFFFFF
-
 
 def level_count(n, r):
     return (n + (1 << r) - 1) >> r
@@ -34,15 +34,19 @@ def build_plan(keys, vals, no_key, nb, L):
             head[k] = q
         if q + 1 == n or keys[q + 1] != k:
             tail[k] = q + 1
-    off = [[0] * (nb + 1) for _ in range(L + 1)]             # k_level_blocksums / scan / offsets
-    for r in range(L + 1):
+    off = [[0] * (nb + 1) for _ in range(2 * L + 1)]         # k_level_blocksums / scan / offsets
+    for row in range(2 * L + 1):
         acc = 0
         for b in range(nb):
-            off[r][b] = acc
-            acc += level_count(tail[b] - head[b], r)
-        off[r][nb] = acc
-    plan0 = [None] * off[1][nb] if L >= 1 else []
-    plan = [None] + [[None] * off[r + 1][nb] for r in range(1, L)]
+            off[row][b] = acc
+            cnt = tail[b] - head[b]
+            acc += level_count(cnt, row) if row <= L else level_count(cnt, row - L - 1) & 1
+        off[row][nb] = acc
+    ncopies = [off[L + 1 + r][nb] for r in range(L)]
+    npairs = [off[r + 1][nb] - ncopies[r] for r in range(L)]
+    pairs = [[None] * npairs[r] for r in range(L)]
+    pair_out = [[None] * npairs[r] for r in range(L)]
+    copies = [[None] * ncopies[r] for r in range(L)]
     surv_keys, surv_vals = [None] * off[L][nb], [None] * off[L][nb]
     for q in range(n):                                      # k_affine_plan
         b = keys[q]
@@ -55,27 +59,33 @@ def build_plan(keys, vals, no_key, nb, L):
                 break
             p = off[r + 1][b] + (i >> (r + 1))
             s = i >> r
-            has2 = s + 1 < level_count(cnt, r)
-            if r == 0:
-                assert plan0[p] is None
-                plan0[p] = (vals[q], vals[q + 1] if has2 else NONE)
+            a = vals[q] if r == 0 else off[r][b] + s
+            singles_before = off[L + 1 + r][b]
+            if s + 1 < level_count(cnt, r):
+                k = p - singles_before
+                assert pairs[r][k] is None
+                pairs[r][k] = (a, vals[q + 1]) if r == 0 else a
+                pair_out[r][k] = p
             else:
-                assert plan[r][p] is None
-                plan[r][p] = (off[r][b] + s) | (0x80000000 if has2 else 0)
+                assert copies[r][singles_before] is None
+                copies[r][singles_before] = (a, p)
         if i & ((1 << L) - 1) == 0:
             ps = off[L][b] + (i >> L)
             assert surv_keys[ps] is None
             surv_keys[ps], surv_vals[ps] = b, ps
-    assert all(x is not None for x in plan0) and all(x is not None for lv in plan[1:] for x in lv)
+    assert all(x is not None for lv in pairs + pair_out + copies for x in lv)
     assert all(x is not None for x in surv_keys)
-    return off, plan0, plan, surv_keys, surv_vals
+    return off, (pairs, pair_out, copies), surv_keys, surv_vals
 
 
-def affine_pairs(cv, first, plan, total, src, threads, stats):
-    """k_affine_pairs: `threads` lanes (multiple of 32), slots split evenly, warp-contiguous ranges."""
+def affine_pairs(cv, first, pairs, pair_out, copies, size, src, threads, stats):
+    """k_affine_pairs: `threads` lanes (multiple of 32), the pair list split evenly in warp-contiguous ranges, then the copy list
+    strided over all lanes. Writes the `size` slots of the next level."""
     p_mod = cv.fp.modulus
     F = pyref
-    dst = [None] * total
+    dst = [None] * size
+    written = [False] * size
+    total = len(pairs)
     M = (total + threads - 1) // threads
 
     def operand(ref):
@@ -84,16 +94,10 @@ def affine_pairs(cv, first, plan, total, src, threads, stats):
             return pyref.ec_neg(P, cv) if (ref >> 31) and P is not None else P
         return src[ref]
 
-    def task(p):
-        if first:
-            return plan[p]
-        v = plan[p]
-        a = v & 0x7FFFFFFF
-        return (a, a + 1 if v >> 31 else NONE)
+    def task(k):
+        return pairs[k] if first else (pairs[k], pairs[k] + 1)
 
-    def classify(single, P1, P2):
-        if single:
-            return "copy1", None
+    def classify(P1, P2):
         if P1 is None:
             return "copy2", None
         if P2 is None:
@@ -118,7 +122,7 @@ def affine_pairs(cv, first, plan, total, src, threads, stats):
         run, prefix = one, []
         for j in range(cnt):
             a, b = task(first_slot + 32 * j)
-            kind, den = classify(b == NONE, operand(a), operand(b) if b != NONE else None)
+            kind, den = classify(operand(a), operand(b))
             if kind in ("add", "dbl"):
                 run = F.f_mul(run, den, p_mod)
             prefix.append(run)
@@ -126,10 +130,10 @@ def affine_pairs(cv, first, plan, total, src, threads, stats):
         inv = F.f_inv(run, p_mod)
         stats["inversions"] += 1
         for j in range(cnt - 1, -1, -1):
-            p = first_slot + 32 * j
-            a, b = task(p)
-            P1, P2 = operand(a), (operand(b) if b != NONE else None)
-            kind, den = classify(b == NONE, P1, P2)
+            k = first_slot + 32 * j
+            a, b = task(k)
+            P1, P2 = operand(a), operand(b)
+            kind, den = classify(P1, P2)
             if kind == "copy1":
                 R = P1
             elif kind == "copy2":
@@ -149,21 +153,24 @@ def affine_pairs(cv, first, plan, total, src, threads, stats):
                 y3 = F.f_sub(F.f_mul(lam, F.f_sub(P1[0], x3, p_mod), p_mod), P1[1], p_mod)
                 R = (x3, y3)
                 stats["adds"] += 1
-            assert dst[p] is None
-            dst[p] = R
+            p = pair_out[k]
+            assert not written[p]
+            dst[p], written[p] = R, True
             stats["slots"] += 1
-    assert stats["slots"] >= total
+    for a, p in copies:                                   # copy_singles
+        assert not written[p]
+        dst[p], written[p] = operand(a), True
+        stats["copies"] += 1
+    assert all(written)
     return dst
 
 
 def run_case(cv, keys, vals, points, no_key, nb, L, threads=64):
-    off, plan0, plan, skeys, svals = build_plan(keys, vals, no_key, nb, L)
-    stats = {"inversions": 0, "adds": 0, "slots": 0}
+    off, (pairs, pair_out, copies), skeys, svals = build_plan(keys, vals, no_key, nb, L)
+    stats = {"inversions": 0, "adds": 0, "slots": 0, "copies": 0}
     work = points
     for r in range(L):
-        total = off[r + 1][nb]
-        work = affine_pairs(cv, r == 0, plan0 if r == 0 else plan[r], total, work, threads, stats)
-        assert all(True for _ in work)
+        work = affine_pairs(cv, r == 0, pairs[r], pair_out[r], copies[r], off[r + 1][nb], work, threads, stats)
     # per bucket: survivors sum == entries sum
     want = {}
     for k, v in zip(keys, vals):
@@ -185,7 +192,7 @@ def self_test(seed=5):
     cv = CURVES["bn254_snarks_g1"]
     rnd = random.Random(seed)
     pool = [pyref.ec_mul_fast(rnd.getrandbits(40) | 1, cv.gen, cv) for _ in range(24)] + [None]
-    total = {"inversions": 0, "adds": 0, "slots": 0}
+    total = {"inversions": 0, "adds": 0, "slots": 0, "copies": 0}
     for trial, (nb, n, L) in enumerate([(7, 90, 1), (7, 90, 3), (16, 400, 4), (3, 200, 5), (40, 60, 2), (1, 129, 3)]):
         ents = []
         for _ in range(n):
@@ -199,5 +206,36 @@ def self_test(seed=5):
     return total
 
 
+def bench_table(logn=20, c=16, L=3, seed=0xC770003):
+    """Per pair level r < L of bench.py's BLS12-381 G1 workload: (slots of level r + 1, single slots of level r). The scalars are
+    bench.py's make_inputs stream; the digits are the engine's signed c-bit windows (tools/bench_affine.py window_digits)."""
+    import numpy as np
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
+    from bench_affine import window_digits
+    cv = CURVES["bls12_381_g1"]
+    rng = np.random.default_rng(seed)
+    s = rng.integers(0, 256, size=(1 << logn, 32), dtype=np.uint8)
+    s[:, 31] &= (1 << (cv.scalar_bits - 248)) - 1
+    n_b = np.concatenate([np.bincount(v[v != 0].astype(np.int64)) for v in window_digits(s, cv.fr.bits, c)])
+    n_b = n_b[n_b > 0]
+    out = []
+    for r in range(L):
+        lvl = (n_b + (1 << r) - 1) >> r
+        out.append((int(((lvl + 1) // 2).sum()), int((lvl & 1).sum())))
+    return out
+
+
 if __name__ == "__main__":
-    print(self_test())
+    if "--bench-table" in sys.argv:
+        import argparse
+        ap = argparse.ArgumentParser()
+        ap.add_argument("--bench-table", action="store_true")
+        ap.add_argument("--logn", type=int, default=20)
+        ap.add_argument("--c", type=int, default=16)
+        ap.add_argument("--levels", type=int, default=3)
+        a = ap.parse_args()
+        print("| pair level | slots | single (copy) slots | share |")
+        for r, (slots, singles) in enumerate(bench_table(a.logn, a.c, a.levels)):
+            print(f"| {r} | {slots} | {singles} | {100 * singles / slots:.1f} % |")
+    else:
+        print(self_test())
