@@ -125,6 +125,18 @@ def load():
     lib.ctt_eth_evm_ecrecover.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_evm_ecrecover_batch.argtypes = [vp, vp, vp, sz]
     lib.ctt_b200_eth_evm_ecrecover_batch.restype = ctypes.c_ubyte
+    for nm in ("sha256", "ripemd160", "modexp"):
+        fn = getattr(lib, "ctt_eth_evm_" + nm)
+        fn.argtypes = [vp, sz, vp, sz]
+        fn.restype = ctypes.c_ubyte
+    lib.ctt_eth_evm_modexp_result_size.argtypes = [ctypes.POINTER(ctypes.c_uint64), vp, sz]
+    lib.ctt_eth_evm_modexp_result_size.restype = ctypes.c_ubyte
+    for nm in ("sha256", "ripemd160"):
+        fn = getattr(lib, "ctt_b200_eth_evm_" + nm + "_batch")
+        fn.argtypes = [vp, vp, sz, vp, sz]
+        fn.restype = ctypes.c_ubyte
+    lib.ctt_b200_eth_evm_modexp_batch.argtypes = [vp, vp, vp, vp, sz, vp, sz]
+    lib.ctt_b200_eth_evm_modexp_batch.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_evm_ecops_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)]
     lib.ctt_b200_eth_evm_ecops_last_timing.restype = None
     lib.ctt_b200_test_bn254_pairing.argtypes = [vp, vp, sz, vp]

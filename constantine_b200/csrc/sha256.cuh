@@ -1,6 +1,7 @@
 // SHA-256 (FIPS 180-4) of a 48-byte message for one thread: the versioned hash of a KZG commitment (EIP-4844 kzg_to_versioned_hash,
 // 0x01 || sha256(commitment)[1:]). 48 bytes, the 0x80 pad byte and the 64-bit bit length fit in one 64-byte block, so the digest is
 // one compression of the initial state. The round loop is rolled; the 16-word schedule window stays in registers.
+// sha256_any hashes a message of any length, one thread per message, for the SHA256 precompile (evm_modexp.cu).
 // The host's SHA-256 (eth_kzg_host.hpp) serves the Fiat-Shamir challenges and is separate.
 #pragma once
 #include <cstdint>
@@ -50,6 +51,60 @@ B200_DEV void sha256_48(const uint32_t* msg, uint32_t* h) {
   }
   h[0] = iv[0] + a; h[1] = iv[1] + b; h[2] = iv[2] + c; h[3] = iv[3] + d;
   h[4] = iv[4] + e; h[5] = iv[5] + f; h[6] = iv[6] + g; h[7] = iv[7] + hh;
+}
+
+// One compression of the 64-byte block w (16 big-endian words, consumed as the schedule window) into the state h.
+B200_DEV void compress(uint32_t* h, uint32_t* w) {
+  uint32_t a = h[0], b = h[1], c = h[2], d = h[3], e = h[4], f = h[5], g = h[6], hh = h[7];
+#pragma unroll 1
+  for (int t = 0; t < 64; t += 16) {
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+      if (t > 0) {
+        const uint32_t w1 = w[(j + 1) & 15], w14 = w[(j + 14) & 15];
+        const uint32_t s0 = rotr(w1, 7) ^ rotr(w1, 18) ^ (w1 >> 3), s1 = rotr(w14, 17) ^ rotr(w14, 19) ^ (w14 >> 10);
+        w[j] += s0 + w[(j + 9) & 15] + s1;
+      }
+      const uint32_t t1 = hh + (rotr(e, 6) ^ rotr(e, 11) ^ rotr(e, 25)) + ((e & f) ^ (~e & g)) + __ldg(K + t + j) + w[j];
+      const uint32_t t2 = (rotr(a, 2) ^ rotr(a, 13) ^ rotr(a, 22)) + ((a & b) ^ (a & c) ^ (b & c));
+      hh = g; g = f; f = e; e = d + t1; d = c; c = b; b = a; a = t1 + t2;
+    }
+  }
+  h[0] += a; h[1] += b; h[2] += c; h[3] += d; h[4] += e; h[5] += f; h[6] += g; h[7] += hh;
+}
+
+// SHA-256 of a message of any length (one thread): the blocks are read byte by byte from global memory, with the 0x80 byte, the
+// zeros and the 64-bit bit length of the padding generated in place. h: the digest as 8 big-endian words.
+B200_DEV void sha256_any(const uint8_t* msg, uint64_t len, uint32_t* h) {
+  h[0] = 0x6a09e667u; h[1] = 0xbb67ae85u; h[2] = 0x3c6ef372u; h[3] = 0xa54ff53au;
+  h[4] = 0x510e527fu; h[5] = 0x9b05688cu; h[6] = 0x1f83d9abu; h[7] = 0x5be0cd19u;
+  const uint64_t blocks = (len + 9 + 63) / 64, bits = len * 8;
+#pragma unroll 1
+  for (uint64_t blk = 0; blk < blocks; blk++) {
+    uint32_t w[16];
+    const uint64_t base = 64 * blk;
+    if (base + 64 <= len) {
+#pragma unroll
+      for (int i = 0; i < 16; i++) {
+        const uint8_t* p = msg + base + 4 * i;
+        w[i] = ((uint32_t)__ldg(p) << 24) | ((uint32_t)__ldg(p + 1) << 16) | ((uint32_t)__ldg(p + 2) << 8) | __ldg(p + 3);
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 16; i++) {
+        uint32_t v = 0;
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          const uint64_t at = base + 4 * i + j;
+          const uint32_t byte = at < len ? __ldg(msg + at) : (at == len ? 0x80u : 0u);
+          v = (v << 8) | byte;
+        }
+        w[i] = v;
+      }
+      if (blk + 1 == blocks) { w[14] = (uint32_t)(bits >> 32); w[15] = (uint32_t)bits; }
+    }
+    compress(h, w);
+  }
 }
 
 }  // namespace sha256

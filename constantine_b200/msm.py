@@ -614,9 +614,95 @@ def eth_evm_ecrecover_batch(data: bytes):
     return _eth_evm_records_batch("ctt_b200_eth_evm_ecrecover_batch", data, 128, 32)
 
 
+def eth_evm_sha256(inputs: bytes, out_len: int = 32):
+    """SHA256 (precompile 0x02) through ctt_eth_evm_sha256: any message -> (status name, 32-byte digest)."""
+    return _eth_evm_ecop("sha256", inputs, out_len)
+
+
+def eth_evm_ripemd160(inputs: bytes, out_len: int = 32):
+    """RIPEMD160 (precompile 0x03) through ctt_eth_evm_ripemd160: any message -> (status name, 12 zero bytes || 20-byte digest)."""
+    return _eth_evm_ecop("ripemd160", inputs, out_len)
+
+
+def eth_evm_modexp_result_size(inputs: bytes):
+    """ctt_eth_evm_modexp_result_size: (status name, mL), the output length eth_evm_modexp needs for this input."""
+    inputs = bytes(inputs)
+    v = ctypes.c_uint64(0)
+    st = _lib.load().ctt_eth_evm_modexp_result_size(ctypes.byref(v), inputs, len(inputs))
+    return EVM_STATUS[st], v.value
+
+
+def eth_evm_modexp(inputs: bytes, out_len: int = None):
+    """MODEXP (precompile 0x05) through ctt_eth_evm_modexp: bL || eL || mL (32 bytes each) || base || exponent || modulus ->
+    (status name, b^e mod M in mL big-endian bytes). out_len defaults to result_size's mL (see the header for the rules)."""
+    inputs = bytes(inputs)
+    if out_len is None:
+        st, out_len = eth_evm_modexp_result_size(inputs)
+        if st != "cttEVM_Success":
+            return st, b""
+    return _eth_evm_ecop("modexp", inputs, out_len)
+
+
+def _offsets(calls):
+    k = len(calls)
+    offsets = (ctypes.c_size_t * (k + 1))()
+    for i, c in enumerate(calls):
+        offsets[i + 1] = offsets[i] + len(c)
+    return offsets, b"".join(calls) or b"\0"
+
+
+def _eth_evm_hash_batch(name, calls) -> list:
+    calls = [bytes(c) for c in calls]
+    k = len(calls)
+    if k == 0:
+        return []
+    offsets, data = _offsets(calls)
+    r = ctypes.create_string_buffer(32 * k)
+    st = getattr(_lib.load(), name)(r, data, offsets[k], offsets, k)
+    if st != 0:
+        raise ValueError(EVM_STATUS[st])
+    raw = r.raw
+    return [raw[32 * i:32 * i + 32] for i in range(k)]
+
+
+def eth_evm_sha256_batch(calls) -> list:
+    """k SHA256 calls of any lengths in one pass (ctt_b200_eth_evm_sha256_batch): a list of messages -> a list of 32-byte digests."""
+    return _eth_evm_hash_batch("ctt_b200_eth_evm_sha256_batch", calls)
+
+
+def eth_evm_ripemd160_batch(calls) -> list:
+    """k RIPEMD160 calls in one pass (ctt_b200_eth_evm_ripemd160_batch): a list of messages -> a list of 32-byte outputs."""
+    return _eth_evm_hash_batch("ctt_b200_eth_evm_ripemd160_batch", calls)
+
+
+def eth_evm_modexp_batch(calls, out_lens=None) -> list:
+    """k MODEXP calls of any lengths in one pass (ctt_b200_eth_evm_modexp_batch): a list of inputs -> [(status name, output)].
+    Output lengths default to each call's result_size (0 where that fails); a failed call's output is zeros."""
+    calls = [bytes(c) for c in calls]
+    k = len(calls)
+    if k == 0:
+        return []
+    if out_lens is None:
+        out_lens = []
+        for c in calls:
+            st, n = eth_evm_modexp_result_size(c)
+            out_lens.append(n if st == "cttEVM_Success" else 0)
+    offsets, data = _offsets(calls)
+    r_offsets = (ctypes.c_size_t * (k + 1))()
+    for i, n in enumerate(out_lens):
+        r_offsets[i + 1] = r_offsets[i] + n
+    r = ctypes.create_string_buffer(max(r_offsets[k], 1))
+    statuses = ctypes.create_string_buffer(k)
+    st = _lib.load().ctt_b200_eth_evm_modexp_batch(r, statuses, r_offsets, data, offsets[k], offsets, k)
+    if st != 0:
+        raise ValueError(EVM_STATUS[st])
+    raw = r.raw
+    return [(EVM_STATUS[statuses.raw[i]], raw[r_offsets[i]:r_offsets[i + 1]]) for i in range(k)]
+
+
 def eth_evm_ecops_last_timing() -> dict:
-    """The kernel time (ms, CUDA events) of the calling thread's last call of the curve addition / multiplication or ecrecover
-    entries above; 0 when that call did no device work."""
+    """The kernel time (ms, CUDA events, first kernel to last) of the calling thread's last call of the curve addition /
+    multiplication, ecrecover, SHA256, RIPEMD160 or MODEXP entries above; 0 when that call did no device work."""
     v = ctypes.c_float(0)
     _lib.load().ctt_b200_eth_evm_ecops_last_timing(ctypes.byref(v))
     return {"ms_kernel": v.value}
