@@ -139,6 +139,16 @@ def load():
     lib.ctt_b200_eth_evm_modexp_batch.restype = ctypes.c_ubyte
     lib.ctt_b200_eth_evm_ecops_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)]
     lib.ctt_b200_eth_evm_ecops_last_timing.restype = None
+    for nm, args in (("sign", [vp, vp, vp, sz, ci]), ("verify", [vp, vp, sz, vp]), ("recover_pubkey", [vp, vp, sz, vp, ci]),
+                     ("recover_pubkey_from_digest", [vp, vp, vp, ci]), ("derive_pubkey", [vp, vp]),
+                     ("sign_batch", [vp, vp, vp, vp, sz, vp, sz, ci]), ("verify_batch", [vp, vp, vp, vp, sz, vp, sz]),
+                     ("recover_pubkey_batch", [vp, vp, vp, vp, vp, sz, vp, sz]),
+                     ("recover_pubkey_from_digest_batch", [vp, vp, vp, vp, vp, sz]), ("derive_pubkey_batch", [vp, vp, vp, sz])):
+        fn = getattr(lib, "ctt_b200_eth_ecdsa_" + nm)
+        fn.argtypes = args
+        fn.restype = ci
+    lib.ctt_b200_eth_ecdsa_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 2
+    lib.ctt_b200_eth_ecdsa_last_timing.restype = None
     lib.ctt_b200_test_bn254_pairing.argtypes = [vp, vp, sz, vp]
     lib.ctt_b200_test_bn254_pairing.restype = ci
     lib.ctt_b200_eth_kzg_context_new.argtypes = [vp]

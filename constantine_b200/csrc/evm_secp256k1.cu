@@ -18,65 +18,19 @@
 // returns, and what it would return otherwise. No thread ever loops over candidates.
 //
 // Per batch one engine lease and stream, one kernel (k_evm_ecrecover, one thread per record) that writes the 32-byte outputs and
-// the statuses; ecops::run_records does the copies and the timing.
+// the statuses; ecops::run_records does the copies and the timing. The recovery itself (k1::recover, secp256k1_recover.cuh) is
+// shared with the ECDSA entries of eth_ecdsa.cu.
 #define CTT_B200_BUILDING_LIBRARY
 #include "../../include/ctt_b200_msm.h"
 #include "ecops_kernels.cuh"
 #include "keccak.cuh"
-#include "secp256k1.cuh"
+#include "secp256k1_recover.cuh"
 #include <cstring>
 
 namespace b200 {
 namespace evmk1 {
 
 constexpr size_t IN_BYTES = 128, OUT_BYTES = 32;
-
-B200_DEV bool is_zero8(const uint32_t* w) {
-  uint32_t o = 0;
-#pragma unroll
-  for (int i = 0; i < 8; i++) o |= w[i];
-  return o == 0;
-}
-
-// the constant table [1..8]G of ecops::joint_mul: the j-th point, negated for d < 0 (d in [-8, 8] \ {0})
-struct GTable {
-  static B200_DEV Aff<FpK1> multiple(int d) {
-    const uint32_t* t = k1::G_TABLE + 16 * ((d < 0 ? -d : d) - 1);
-    Aff<FpK1> g;
-#pragma unroll
-    for (int w = 0; w < 8; w++) { g.x.l[w] = __ldg(t + w); g.y.l[w] = __ldg(t + 8 + w); }
-    if (d < 0) g.y = g.y.neg();
-    return g;
-  }
-};
-
-// the recovered key of one well-formed record (affine; (0, 0) when there is none)
-static __device__ __noinline__ Aff<FpK1> recover(const uint8_t* s, bool odd) {
-  uint32_t m[8], r[8], sc[8];
-  ecops::load_scalar(s, m);
-  ecops::load_scalar(s + 64, r);
-  ecops::load_scalar(s + 96, sc);
-  k1::fr_reduce(m);
-  k1::fr_reduce(r);
-  k1::fr_reduce(sc);
-  Aff<FpK1> q;
-  q.x = FpK1::zero();
-  q.y = FpK1::zero();
-  if (is_zero8(r) || is_zero8(sc)) return q;
-  Aff<FpK1> R;
-#pragma unroll
-  for (int w = 0; w < 8; w++) R.x.l[w] = r[w];   // r < n < p
-  const FpK1 alpha = R.x.sqr() * R.x + FpK1::from_u32(k1::B);
-  R.y = k1::fp_sqrt_candidate(alpha);
-  if (!(R.y.sqr() == alpha)) return q;           // x1 does not lift: no key
-  if (((R.y.l[0] & 1u) != 0) != odd) R.y = R.y.neg();
-  uint32_t ri[8], u1[8], u2[8];
-  k1::fr_inv(ri, r);
-  k1::fr_mul(u1, m, ri);
-  k1::fr_neg(u1, u1);
-  k1::fr_mul(u2, sc, ri);
-  return to_affine(ecops::joint_mul<FpK1, GTable>(R, u1, u2));   // R is finite
-}
 
 // src: n records of 128 bytes; out: n x 32 bytes (12 zero bytes, then the 20-byte address; all zeros on MalformedSignature)
 static __global__ void __launch_bounds__(ecops::THREADS) k_evm_ecrecover(const uint8_t* __restrict__ src, size_t n, uint8_t* out,
@@ -96,7 +50,11 @@ static __global__ void __launch_bounds__(ecops::THREADS) k_evm_ecrecover(const u
     status[i] = cttEVM_MalformedSignature;
     return;
   }
-  const Aff<FpK1> q = recover(s, vb == 1 || vb == 28);
+  uint32_t m[8], r[8], sc[8];
+  ecops::load_scalar(s, m);
+  ecops::load_scalar(s + 64, r);
+  ecops::load_scalar(s + 96, sc);
+  const Aff<FpK1> q = k1::recover(m, r, sc, vb == 1 || vb == 28);
   uint32_t msg[16], h[8];   // x || y, 32 big-endian bytes each
 #pragma unroll
   for (int j = 0; j < 8; j++) {

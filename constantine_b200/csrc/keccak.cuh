@@ -75,5 +75,53 @@ B200_DEV void keccak256_64(const uint32_t* m, uint32_t* out) {
   for (int k = 0; k < 4; k++) { out[2 * k] = s[k].x; out[2 * k + 1] = s[k].y; }
 }
 
+// Keccak-256 of a message of any length whose byte i is ld(i) (one thread): blocks of the 136-byte rate, the padding 0x01 ... 0x80
+// generated in place (0x81 when both fall on one byte). Which bytes are read depends on len only. out: 8 little-endian words.
+template <class Ld>
+B200_DEV void keccak256_bytes(Ld ld, uint64_t len, uint32_t* out) {
+  constexpr int RATE = 136, LANES = RATE / 8;
+  uint2 s[25];
+#pragma unroll
+  for (int k = 0; k < 25; k++) s[k] = make_uint2(0u, 0u);
+  const uint64_t blocks = len / RATE + 1;
+#pragma unroll 1
+  for (uint64_t blk = 0; blk < blocks; blk++) {
+    const uint64_t base = RATE * blk;
+    if (base + RATE <= len) {
+#pragma unroll
+      for (int k = 0; k < LANES; k++) {
+        uint32_t w[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const uint64_t at = base + 8 * k + 4 * h;
+          w[h] = (uint32_t)ld(at) | ((uint32_t)ld(at + 1) << 8) | ((uint32_t)ld(at + 2) << 16) | ((uint32_t)ld(at + 3) << 24);
+        }
+        s[k] = x2(s[k], make_uint2(w[0], w[1]));
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < LANES; k++) {
+        uint32_t w[2] = {0u, 0u};
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+          const uint64_t at = base + 8 * k + j;
+          const uint32_t byte = at < len ? (uint32_t)ld(at) : (at == len ? 0x01u : 0u);
+          w[j >> 2] |= byte << (8 * (j & 3));
+        }
+        s[k] = x2(s[k], make_uint2(w[0], w[1]));
+      }
+      s[LANES - 1].y ^= 0x80000000u;   // the last byte of the rate, in the last block
+    }
+    f1600(s);
+  }
+#pragma unroll
+  for (int k = 0; k < 4; k++) { out[2 * k] = s[k].x; out[2 * k + 1] = s[k].y; }
+}
+
+// Keccak-256 of msg[0, len) in global memory (one thread), read byte by byte through the read-only cache
+B200_DEV void keccak256_any(const uint8_t* msg, uint64_t len, uint32_t* out) {
+  keccak256_bytes([=](uint64_t i) { return __ldg(msg + i); }, len, out);
+}
+
 }  // namespace keccak
 }  // namespace b200

@@ -12,7 +12,8 @@
 // Scalar field: values < n in the same form. The few operations of a record: reduction of a 256-bit value (one conditional
 // subtraction, 2^256 < 2n), products (the same 512-bit product folded with C = 2^256 - n < 2^129 until it fits 256 bits),
 // negation (field.cuh's fe_neg) and safegcd inversion over Secp256k1Fr.
-// Not constant time: every input of a precompile is public.
+// Not constant time: every input of a precompile is public. The signing kernels use secp256k1_ct.cuh, which takes mul_wide and the
+// folds with CT = true: their last reduction is then cond_sub_ct, a select by masks instead of a branch on the carry.
 #pragma once
 #include "field.cuh"
 #include "field_inv.cuh"
@@ -70,8 +71,30 @@ B200_DEV void cond_sub(uint32_t* r, const uint32_t* x, uint32_t carry) {
   for (int i = 0; i < 8; i++) r[i] = take ? t[i] : x[i];
 }
 
+// cond_sub with no branch and no select on the data: the borrow and the carry become masks
+template <class F>
+B200_DEV void cond_sub_ct(uint32_t* r, const uint32_t* x, uint32_t carry) {
+  uint32_t t[8];
+  t[0] = p_sub_cc(x[0], F::P(0));
+#pragma unroll
+  for (int i = 1; i < 8; i++) t[i] = p_subc_cc(x[i], F::P(i));
+  const uint32_t keep = p_subc(0, 0) & (carry - 1u);   // x < m and no carry: all ones
+#pragma unroll
+  for (int i = 0; i < 8; i++) r[i] = (x[i] & keep) | (t[i] & ~keep);
+}
+
+template <bool CT>
+B200_DEV void cond_sub_p(uint32_t* r, const uint32_t* x) {
+  if constexpr (CT) cond_sub_ct<Secp256k1Fp>(r, x, 0); else cond_sub<Secp256k1Fp>(r, x, 0);
+}
+template <bool CT>
+B200_DEV void cond_sub_n(uint32_t* r, const uint32_t* x) {
+  if constexpr (CT) cond_sub_ct<Secp256k1Fr>(r, x, 0); else cond_sub<Secp256k1Fr>(r, x, 0);
+}
+
 // r = T mod p for the 512-bit product T: T = H 2^256 + L = L + 977 H + 2^32 H (below 2^289), then its top 33 bits are folded the
 // same way (below 2^256 + 2^67), then a final wrap by C and one conditional subtraction.
+template <bool CT = false>
 B200_DEV void fold_p(uint32_t* r, const uint32_t* T) {
   uint32_t R[8], r8, r9;
   R[0] = p_mad_lo_cc(T[8], 977u, T[0]);
@@ -103,11 +126,12 @@ B200_DEV void fold_p(uint32_t* r, const uint32_t* T) {
 #pragma unroll
   for (int j = 2; j < 7; j++) R[j] = p_addc_cc(R[j], 0);
   R[7] = p_addc(R[7], 0);
-  cond_sub<Secp256k1Fp>(r, R, 0);
+  cond_sub_p<CT>(r, R);
 }
 
 // r = T mod n for the 512-bit product T, folding with C = 2^256 - n (5 words, < 2^129): L + H C < 2^386, then its top 130 bits
 // (< 2^260), then its top 4 bits (< 2^257), then the carry once more (< 2^256 after it), then one conditional subtraction.
+template <bool CT = false>
 B200_DEV void fold_n(uint32_t* r, const uint32_t* T) {
   using F = Secp256k1Fr;
   static_assert(F::NC == 5, "C = 2^256 - n has 129 bits");
@@ -136,7 +160,7 @@ B200_DEV void fold_n(uint32_t* r, const uint32_t* T) {
   h = Y[8];
   Y[8] = 0;
   row_acc<10, 5, 0>(Y, c, h);
-  cond_sub<F>(r, Y, 0);
+  cond_sub_n<CT>(r, Y);
 }
 
 }  // namespace k1

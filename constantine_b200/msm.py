@@ -614,6 +614,117 @@ def eth_evm_ecrecover_batch(data: bytes):
     return _eth_evm_records_batch("ctt_b200_eth_evm_ecrecover_batch", data, 128, 32)
 
 
+ECDSA_STATUS = ("cttEthEcdsa_Success", "cttEthEcdsa_VerificationFailure", "cttEthEcdsa_SecretKeyOutOfRange",
+                "cttEthEcdsa_SignatureOutOfRange", "cttEthEcdsa_PublicKeyCoordinateOutOfRange", "cttEthEcdsa_PublicKeyNotOnCurve",
+                "cttEthEcdsa_NonceFailure")
+ECDSA_NONCE = {"random": 0, "rfc6979": 1}   # the reference's NonceSampler order
+
+
+def _ecdsa_call(name, *args):
+    rc = getattr(_lib.load(), "ctt_b200_eth_ecdsa_" + name)(*args)
+    if rc < 0:
+        raise ValueError("ctt_b200_eth_ecdsa_%s: invalid call" % name)
+    return rc
+
+
+def _ecdsa_one(name, out_size, *args):
+    out = ctypes.create_string_buffer(out_size)
+    return ECDSA_STATUS[_ecdsa_call(name, out, *args)], out.raw
+
+
+def eth_ecdsa_sign(seckey: bytes, msg: bytes, nonce: str = "rfc6979"):
+    """Ethereum ECDSA signature of msg (hashed with Keccak-256) under the 32-byte big-endian secret key, through
+    ctt_b200_eth_ecdsa_sign: (status name, r || s, 64 bytes, low s). nonce: "rfc6979" (deterministic) or "random"."""
+    msg = bytes(msg)
+    return _ecdsa_one("sign", 64, bytes(seckey), msg, len(msg), ECDSA_NONCE[nonce])
+
+
+def eth_ecdsa_verify(pubkey: bytes, msg: bytes, sig: bytes) -> str:
+    """ctt_b200_eth_ecdsa_verify: the status of sig (r || s) over msg under the 64-byte key x || y."""
+    msg = bytes(msg)
+    return ECDSA_STATUS[_ecdsa_call("verify", bytes(pubkey), msg, len(msg), bytes(sig))]
+
+
+def eth_ecdsa_recover_pubkey(msg: bytes, sig: bytes, even_y: bool):
+    """ctt_b200_eth_ecdsa_recover_pubkey: (status name, the 64-byte key; zeros when there is none)."""
+    msg = bytes(msg)
+    return _ecdsa_one("recover_pubkey", 64, msg, len(msg), bytes(sig), int(bool(even_y)))
+
+
+def eth_ecdsa_recover_pubkey_from_digest(digest: bytes, sig: bytes, even_y: bool):
+    """ctt_b200_eth_ecdsa_recover_pubkey_from_digest: a 32-byte digest (taken mod n) instead of the message."""
+    return _ecdsa_one("recover_pubkey_from_digest", 64, bytes(digest), bytes(sig), int(bool(even_y)))
+
+
+def eth_ecdsa_derive_pubkey(seckey: bytes):
+    """ctt_b200_eth_ecdsa_derive_pubkey: (status name, [d]G as x || y)."""
+    return _ecdsa_one("derive_pubkey", 64, bytes(seckey))
+
+
+def _ecdsa_joined(items, size, n):
+    items = [bytes(x) for x in items]
+    if len(items) != n or any(len(x) != size for x in items):
+        raise ValueError("%d items of %d bytes expected" % (n, size))
+    return b"".join(items)
+
+
+def _ecdsa_messages(msgs):
+    offsets, data = _offsets([bytes(m) for m in msgs])
+    return data, offsets[len(msgs)], offsets
+
+
+def _ecdsa_batch(name, n, out_size, *args):
+    """n items through ctt_b200_eth_ecdsa_<name>_batch: [(status name, out_size output bytes)], or [status name] for out_size 0"""
+    if n == 0:
+        return []
+    st = ctypes.create_string_buffer(n)
+    if not out_size:
+        _ecdsa_call(name + "_batch", st, *args)
+        return [ECDSA_STATUS[b] for b in st.raw]
+    out = ctypes.create_string_buffer(out_size * n)
+    _ecdsa_call(name + "_batch", out, st, *args)
+    return [(ECDSA_STATUS[st.raw[i]], out.raw[out_size * i:out_size * (i + 1)]) for i in range(n)]
+
+
+def eth_ecdsa_sign_batch(seckeys, msgs, nonce: str = "rfc6979") -> list:
+    """n signatures in one pass (ctt_b200_eth_ecdsa_sign_batch): lists of secret keys and messages -> [(status name, r || s)]."""
+    n = len(msgs)
+    return _ecdsa_batch("sign", n, 64, _ecdsa_joined(seckeys, 32, n), *_ecdsa_messages(msgs), n, ECDSA_NONCE[nonce])
+
+
+def eth_ecdsa_verify_batch(pubkeys, msgs, sigs) -> list:
+    """n verifications in one pass (ctt_b200_eth_ecdsa_verify_batch) -> [status name]."""
+    n = len(msgs)
+    return _ecdsa_batch("verify", n, 0, _ecdsa_joined(pubkeys, 64, n), _ecdsa_joined(sigs, 64, n), *_ecdsa_messages(msgs), n)
+
+
+def eth_ecdsa_recover_pubkey_batch(msgs, sigs, even_y) -> list:
+    """n recoveries in one pass (ctt_b200_eth_ecdsa_recover_pubkey_batch) -> [(status name, 64-byte key)]."""
+    n = len(msgs)
+    ev = _ecdsa_joined([b"\1" if e else b"\0" for e in even_y], 1, n)
+    return _ecdsa_batch("recover_pubkey", n, 64, _ecdsa_joined(sigs, 64, n), ev, *_ecdsa_messages(msgs), n)
+
+
+def eth_ecdsa_recover_pubkey_from_digest_batch(digests, sigs, even_y) -> list:
+    """n recoveries from 32-byte digests in one pass (ctt_b200_eth_ecdsa_recover_pubkey_from_digest_batch)."""
+    n = len(digests)
+    ev = _ecdsa_joined([b"\1" if e else b"\0" for e in even_y], 1, n)
+    return _ecdsa_batch("recover_pubkey_from_digest", n, 64, _ecdsa_joined(digests, 32, n), _ecdsa_joined(sigs, 64, n), ev, n)
+
+
+def eth_ecdsa_derive_pubkey_batch(seckeys) -> list:
+    """n public keys in one pass (ctt_b200_eth_ecdsa_derive_pubkey_batch) -> [(status name, x || y)]."""
+    n = len(seckeys)
+    return _ecdsa_batch("derive_pubkey", n, 64, _ecdsa_joined(seckeys, 32, n), n)
+
+
+def eth_ecdsa_last_timing() -> dict:
+    """The calling thread's last ECDSA call: host work before the kernel and the kernel's CUDA-event time (ms)."""
+    h, k = ctypes.c_float(0), ctypes.c_float(0)
+    _lib.load().ctt_b200_eth_ecdsa_last_timing(ctypes.byref(h), ctypes.byref(k))
+    return {"ms_host": h.value, "ms_kernel": k.value}
+
+
 def eth_evm_sha256(inputs: bytes, out_len: int = 32):
     """SHA256 (precompile 0x02) through ctt_eth_evm_sha256: any message -> (status name, 32-byte digest)."""
     return _eth_evm_ecop("sha256", inputs, out_len)

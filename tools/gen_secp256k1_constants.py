@@ -1,5 +1,6 @@
 #!/usr/bin/env python3
-"""Derive the secp256k1 constants of the ecrecover kernel and write constantine_b200/csrc/secp256k1_constants.cuh.
+"""Derive the secp256k1 constants of the ecrecover and ECDSA kernels and write constantine_b200/csrc/secp256k1_constants.cuh and
+constantine_b200/csrc/secp256k1_ct_table.cuh (the second is not kept in git: the library's Makefile runs this script to make it).
 
 Every value is computed here from p, n, b = 7 and the generator G (SEC 2, section 2.4.1); nothing is copied from a table. The script
 asserts what the kernel relies on:
@@ -10,6 +11,9 @@ asserts what the kernel relies on:
   - the safegcd constants: 9 signed 30-bit limbs hold (-2m, m), and floor((45907 * 256 + 26313) / 19929) = 591 divsteps, i.e. 20
     batches of 30, always suffice.
 Both fields are kept in plain (non-Montgomery) form, so the inversion starts from e = 1 (R2_30 below) and returns a^-1 itself.
+The signing kernels' fixed-base table (secp256k1_ct.cuh) holds [j 16^i]G for 64 windows i and j = 1..15, built by repeated
+addition of G and 16^i G; every entry is checked on the curve and against an independent double-and-add [j 16^i]G, and no entry
+is infinity (j 16^i < n), so the complete addition's (0 : 1 : 0) for a zero digit is the only infinity the kernel selects.
 """
 import os
 import sys
@@ -22,6 +26,8 @@ B = 7
 GX = 0x79BE667EF9DCBBAC55A06295CE870B07029BFCDB2DCE28D959F2815B16F81798
 GY = 0x483ADA7726A3C4655DA4FBFC0E1108A8FD17B448A68554199C47D08FFB10D4B8
 TABLE = 8            # [1..TABLE]G for the signed 4-bit digits of the joint multiplication
+OUT_CT = os.path.join(ROOT, "constantine_b200", "csrc", "secp256k1_ct_table.cuh")
+CT_WINDOWS, CT_ENTRIES = 64, 15   # [j 16^i]G, i < 64, j = 1..15: one complete addition per 4-bit window of a 256-bit scalar
 
 
 def ec_add(a, b):
@@ -141,6 +147,42 @@ def header_text():
     return "\n".join(lines)
 
 
+def ct_table():
+    """rows[i][j - 1] = [j 16^i]G, checked against double-and-add"""
+    rows, base = [], (GX, GY)
+    for i in range(CT_WINDOWS):
+        row, acc = [], None
+        for j in range(1, CT_ENTRIES + 1):
+            acc = ec_add(acc, base)
+            assert acc is not None and j * 16 ** i < N
+            assert (acc[1] ** 2 - acc[0] ** 3 - B) % P == 0
+            row.append(acc)
+        assert row[5] == ec_mul(6 * 16 ** i, (GX, GY)) and row[-1] == ec_mul(15 * 16 ** i, (GX, GY))
+        rows.append(row)
+        base = ec_add(row[-1], base)
+    return rows
+
+
+def ct_header_text():
+    tw = [w for row in ct_table() for (x, y) in row for w in words(x) + words(y)]
+    lines = [
+        "// GENERATED by tools/gen_secp256k1_constants.py -- the fixed-base table of the secp256k1 signing kernels, see that file.",
+        "// Entry (i, j), i < %d, j = 1..%d: [j 16^i]G affine, x then y as 8 plain little-endian words each, at 16 (%d i + j - 1)."
+        % (CT_WINDOWS, CT_ENTRIES, CT_ENTRIES),
+        "#pragma once",
+        "#include <cstdint>",
+        "",
+        "namespace b200 {",
+        "namespace k1 {",
+        "constexpr int CT_WINDOWS = %d, CT_ENTRIES = %d;" % (CT_WINDOWS, CT_ENTRIES),
+        "static __device__ const uint32_t CT_G_TABLE[%d] = {" % len(tw),
+    ]
+    for k in range(0, len(tw), 8):
+        lines.append("    " + ", ".join("0x%08xu" % w for w in tw[k:k + 8]) + ",")
+    lines += ["};", "}  // namespace k1", "}  // namespace b200", ""]
+    return "\n".join(lines)
+
+
 def write_if_changed(path, text):
     if os.path.exists(path) and open(path).read() == text:
         return False
@@ -151,5 +193,6 @@ def write_if_changed(path, text):
 
 if __name__ == "__main__":
     check()
-    changed = write_if_changed(OUT, header_text())
-    print("%s %s" % ("wrote" if changed else "unchanged", os.path.relpath(OUT, ROOT)), file=sys.stderr)
+    for path, text in ((OUT, header_text()), (OUT_CT, ct_header_text())):
+        changed = write_if_changed(path, text)
+        print("%s %s" % ("wrote" if changed else "unchanged", os.path.relpath(path, ROOT)), file=sys.stderr)
