@@ -228,6 +228,15 @@ def load():
     lib.ctt_b200_eth_bls_deserialize_signatures_compressed_batch.restype = ci
     lib.ctt_b200_eth_bls_registry_from_compressed.argtypes = [vp, sz, vp, ctypes.POINTER(sz), ctypes.POINTER(ci)]
     lib.ctt_b200_eth_bls_registry_from_compressed.restype = vp
+    for nm, args in (("sign", [vp, vp, vp, sz]), ("sign_batch", [vp, vp, vp, vp, sz, vp, sz]), ("derive_pubkey", [vp, vp]),
+                     ("derive_pubkey_batch", [vp, vp, vp, sz]), ("serialize_pubkey_compressed", [vp, vp]),
+                     ("serialize_signature_compressed", [vp, vp]), ("serialize_pubkeys_compressed_batch", [vp, vp, sz]),
+                     ("serialize_signatures_compressed_batch", [vp, vp, sz])):
+        fn = getattr(lib, "ctt_b200_eth_bls_" + nm)
+        fn.argtypes = args
+        fn.restype = ci
+    lib.ctt_b200_eth_bls_signer_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 3
+    lib.ctt_b200_eth_bls_signer_last_timing.restype = None
     lib.ctt_b200_fft_domain_new.argtypes = [ci, vp, ci, ctypes.POINTER(ci)]
     lib.ctt_b200_fft_domain_new.restype = vp
     lib.ctt_b200_fft_domain_free.argtypes = [vp]

@@ -22,6 +22,7 @@
 #include "bls_sets_kernels.cuh"
 #include "codec_kernels.cuh"
 #include "pairing_check.cuh"
+#include "eth_bls_host.hpp"
 #include "eth_kzg_host.hpp"
 #include "host_pairing.hpp"
 #include <algorithm>
@@ -44,8 +45,7 @@ enum Status : uint8_t { Success = 0, VerificationFailure = 1, InputsLengthsMisma
 enum CodecStatus : int { CodecSuccess = 0, CodecInvalidEncoding = 1, CodecCoordinateGeqModulus = 2, CodecNotOnCurve = 3,
                          CodecNotInSubgroup = 4, CodecPointAtInfinity = 5 };
 
-struct Span { const uint8_t* data; size_t len; };   // ctt_span
-constexpr size_t PK_BYTES = 96, SIG_BYTES = 192, UNIFORM_BYTES = 256;
+constexpr size_t PK_BYTES = 96, SIG_BYTES = 192;
 static const char POP_DST[] = "BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_POP_";
 
 struct Timing { float ms_host = 0, ms_hash = 0, ms_blind = 0, ms_msm = 0, ms_miller = 0, ms_final = 0; };
@@ -64,7 +64,6 @@ static bool all_zero(const uint8_t* p, size_t n) {
   return o == 0;
 }
 
-// RFC 9380 section 5.3.1 with SHA-256 and len_in_bytes = 256 (ell = 8)
 void expand_message_xmd(uint8_t out[UNIFORM_BYTES], const uint8_t* msg, size_t msg_len, const uint8_t* dst, size_t dst_len) {
   static const uint8_t z_pad[64] = {0};
   const uint8_t lib[2] = {(uint8_t)(UNIFORM_BYTES >> 8), (uint8_t)UNIFORM_BYTES}, dlen = (uint8_t)dst_len;
@@ -108,7 +107,7 @@ void blinding_chain(uint64_t* r, size_t n, const uint8_t secure_random_bytes[32]
   }
 }
 
-static void expand_all(std::vector<uint8_t>& uniform, const Span* messages, size_t n) {
+void expand_all(std::vector<uint8_t>& uniform, const Span* messages, size_t n) {
   uniform.resize(n * UNIFORM_BYTES);
   kzg::parallel_for(n, [&](size_t i) {
     expand_message_xmd(&uniform[UNIFORM_BYTES * i], messages[i].data, messages[i].len, (const uint8_t*)POP_DST, sizeof(POP_DST) - 1);

@@ -1,0 +1,412 @@
+// Ethereum BLS signing (proof-of-possession scheme, signatures in G2) on the GPU: the reference's sign, derive_pubkey and
+// serialize_{pubkey,signature}_compressed (constantine/ethereum_bls_signatures.nim:133-234, coreSign at
+// signatures/bls_signatures.nim:40-77, codecs at serialization/codecs_bls12_381.nim:59-219) as byte entries with this library's
+// prefix, single and batched, DESIGN §4w. Secret keys are 32 big-endian bytes, public keys 48 compressed bytes, signatures 96.
+//
+// One thread per item in each kernel:
+//   k_bls_sign      the key's range check, the table [1..15]H(m) from the hash kernel's H(m) (public: variable-time ec.cuh code and
+//                   one inversion), then [sk]H(m) with blsct::ct_mul_g2, its affine form and compression;
+//   k_bls_derive    the key's range check, [sk]G1 with blsct::ct_fixed_base_g1, compression;
+//   k_bls_serialize_g1 / _g2   affine Montgomery structs ((0, 0) is infinity) to the compressed formats.
+// Signing runs the existing k_bls_hash_to_g2 first; expand_message_xmd runs on the host (eth_bls_host.hpp).
+// Host: per batch one engine lease and stream, one upload, the kernels, one copy back. Device buffers that held secret keys are
+// zeroed on the stream before they are freed.
+#define CTT_B200_BUILDING_LIBRARY
+#include "../../include/ctt_b200_msm.h"
+#include "msm_hooks.cuh"
+#include "h2c_kernels.cuh"
+#include "bls_ct.cuh"
+#include "eth_bls_host.hpp"
+#include "host_bls12_381.hpp"
+#include <chrono>
+#include <cstring>
+#include <initializer_list>
+#include <vector>
+
+namespace b200 {
+namespace blssign {
+
+using bls::Fq;
+using bls::Fq2;
+
+constexpr int THREADS = 64;
+constexpr size_t SK_BYTES = 32, PK_BYTES = 48, SIG_BYTES = 96, G1_AFF = 96, G2_AFF = 192, LIMIT = size_t(1) << 31;
+// ctt_codec_scalar_status
+enum ScalarStatus : uint8_t { ScalarSuccess = 0, ScalarZero = 1, ScalarLargerThanCurveOrder = 2 };
+
+// ---- device helpers ---------------------------------------------------------------------------------------------------------
+// 32 big-endian bytes (16-byte aligned) -> 8 little-endian words
+B200_DEV void load_be32(const uint8_t* s, uint32_t* w) {
+  const uint4* q = reinterpret_cast<const uint4*>(s);
+#pragma unroll
+  for (int k = 0; k < 2; k++) {
+    const uint4 v = __ldg(q + k);
+    w[7 - 4 * k] = __byte_perm(v.x, 0, 0x0123);
+    w[6 - 4 * k] = __byte_perm(v.y, 0, 0x0123);
+    w[5 - 4 * k] = __byte_perm(v.z, 0, 0x0123);
+    w[4 - 4 * k] = __byte_perm(v.w, 0, 0x0123);
+  }
+}
+// 12 little-endian words -> 48 big-endian bytes (16-byte aligned)
+B200_DEV void store_be48(uint8_t* d, const uint32_t* w) {
+  uint4* q = reinterpret_cast<uint4*>(d);
+#pragma unroll
+  for (int k = 0; k < 3; k++)
+    q[k] = make_uint4(__byte_perm(w[11 - 4 * k], 0, 0x0123), __byte_perm(w[10 - 4 * k], 0, 0x0123),
+                      __byte_perm(w[9 - 4 * k], 0, 0x0123), __byte_perm(w[8 - 4 * k], 0, 0x0123));
+}
+B200_DEV void store_zero(uint8_t* d, int bytes) {
+  uint4* q = reinterpret_cast<uint4*>(d);
+  for (int k = 0; k < bytes / 16; k++) q[k] = make_uint4(0, 0, 0, 0);
+}
+// 0xC0 then zeros
+B200_DEV void store_infinity(uint8_t* d, int bytes) {
+  store_zero(d, bytes);
+  d[0] = 0xC0;
+}
+
+// deserialize_seckey's status: 0 for k in [1, r - 1], 1 for k = 0, 2 for k >= r (the reference's validate_scalar, which also
+// branches on these)
+B200_DEV uint8_t scalar_status(const uint32_t* k) {
+  uint32_t any = 0, r[8], t[8];
+#pragma unroll
+  for (int w = 0; w < 8; w++) { any |= k[w]; r[w] = Bls12381Fr::P(w); }
+  const uint32_t below = limbs_sub<8>(t, k, r);
+  return any == 0 ? ScalarZero : below ? ScalarSuccess : ScalarLargerThanCurveOrder;
+}
+
+// canonical words of a Montgomery element
+B200_DEV Fq canonical(const Fq& a) { return bls::from_mont(a); }
+// all ones when the canonical a is above (p - 1) / 2, else 0
+B200_DEV uint32_t above_half(const Fq& a) {
+  uint32_t h[12], t[12];
+  bls::p_minus_shift(h, 1, 1);
+  return limbs_sub<12>(t, h, a.l);
+}
+
+// The compressed formats (host_bls12_381.hpp compress_g1 / compress_g2, the reference's serializers); the flags are computed on the
+// public output. G1: 0x20 for y >= (p - 1) / 2.
+B200_DEV void compress_g1(uint8_t* out, const Fq& x, const Fq& y) {
+  if (x.is_zero() && y.is_zero()) { store_infinity(out, 48); return; }
+  Fq cx = canonical(x);
+  const Fq cy = canonical(y);
+  uint32_t h[12], t[12];
+  bls::p_minus_shift(h, 1, 1);
+  const bool large = limbs_sub<12>(t, cy.l, h) == 0;
+  cx.l[11] |= (0x80u | (large ? 0x20u : 0u)) << 24;
+  store_be48(out, cx.l);
+}
+// G2: x.c1 then x.c0; 0x20 for y.c1 > (p - 1) / 2, or y.c0 > (p - 1) / 2 when y.c1 = 0
+B200_DEV void compress_g2(uint8_t* out, const Fq2& x, const Fq2& y) {
+  if (x.is_zero() && y.is_zero()) { store_infinity(out, 96); return; }
+  Fq c1 = canonical(x.c1);
+  const Fq c0 = canonical(x.c0);
+  const bool large = (y.c1.is_zero() ? above_half(canonical(y.c0)) : above_half(canonical(y.c1))) != 0;
+  c1.l[11] |= (0x80u | (large ? 0x20u : 0u)) << 24;
+  store_be48(out, c1.l);
+  store_be48(out + 48, c0.l);
+}
+
+// ---- kernels ------------------------------------------------------------------------------------------------------------------
+// pubs[48 i, +48) = compress([sk_i]G1) for sks[32 i, +32); 48 zero bytes when status[i] != 0
+static __global__ void __launch_bounds__(THREADS) k_bls_derive(const uint8_t* __restrict__ sks, size_t n, uint8_t* pubs, uint8_t* status) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint8_t* o = pubs + PK_BYTES * i;
+  uint32_t k[8];
+  load_be32(sks + SK_BYTES * i, k);
+  const uint8_t st = scalar_status(k);
+  if (st != ScalarSuccess) {   // the key's validity is what the status reports
+    store_zero(o, PK_BYTES);
+    status[i] = st;
+    return;
+  }
+  Fq x, y;
+  blsct::ct_fixed_base_g1(x, y, k);
+  compress_g1(o, x, y);
+  status[i] = ScalarSuccess;
+}
+
+// sigs[96 i, +96) = compress([sk_i]H_i) for H_i = hashes[i] (affine G2 from k_bls_hash_to_g2) and sks[32 i, +32); 96 zero bytes when
+// status[i] != 0
+static __global__ void __launch_bounds__(THREADS) k_bls_sign(const uint32_t* hashes, const uint8_t* __restrict__ sks, size_t n,
+                                                             uint8_t* sigs, uint8_t* status) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint8_t* o = sigs + SIG_BYTES * i;
+  uint32_t k[8];
+  load_be32(sks + SK_BYTES * i, k);
+  const uint8_t st = scalar_status(k);
+  if (st != ScalarSuccess) {
+    store_zero(o, SIG_BYTES);
+    status[i] = st;
+    return;
+  }
+  Aff<Fq2> h;
+  load_words_rw(h.x, hashes + i * 2 * Fq2::WORDS);
+  load_words_rw(h.y, hashes + i * 2 * Fq2::WORDS + Fq2::WORDS);
+  status[i] = ScalarSuccess;
+  if (h.is_inf()) {   // public: [sk]O = O
+    store_infinity(o, SIG_BYTES);
+    return;
+  }
+  // tab[j] = [j]H, j = 1..15, public: XYZZ sums, then affine with one inversion for all (Montgomery's trick on d_j = ZZ_j ZZZ_j,
+  // x_j = X_j ZZZ_j / d_j, y_j = Y_j ZZ_j / d_j). H has order r, so no d_j is zero.
+  Aff<Fq2> tab[16];
+  Fq2 d[16], pre[16];
+  Xyzz<Fq2> acc = Xyzz<Fq2>::from_affine(h);
+#pragma unroll 1
+  for (int j = 1; j <= 15; j++) {
+    if (j > 1) xyzz_madd_ni(acc, h);
+    tab[j].x = acc.x * acc.zzz;
+    tab[j].y = acc.y * acc.zz;
+    d[j] = acc.zz * acc.zzz;
+    pre[j] = j == 1 ? d[j] : pre[j - 1] * d[j];
+  }
+  Fq2 inv = fe_inverse(pre[15]);
+#pragma unroll 1
+  for (int j = 15; j >= 1; j--) {
+    const Fq2 dj = j > 1 ? inv * pre[j - 1] : inv;
+    inv = inv * d[j];
+    tab[j].x = tab[j].x * dj;
+    tab[j].y = tab[j].y * dj;
+  }
+  Fq2 x, y;
+  blsct::ct_mul_g2(x, y, tab, k);
+  compress_g2(o, x, y);
+}
+
+// out[48 i, +48) (G1) or out[96 i, +96) (G2) = the compressed form of the affine Montgomery struct pts[i]
+static __global__ void __launch_bounds__(128) k_bls_serialize_g1(const uint32_t* __restrict__ pts, size_t n, uint8_t* out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  Aff<Fq> a;
+  load_words(a.x, pts + i * 2 * Fq::WORDS);
+  load_words(a.y, pts + i * 2 * Fq::WORDS + Fq::WORDS);
+  compress_g1(out + PK_BYTES * i, a.x, a.y);
+}
+static __global__ void __launch_bounds__(128) k_bls_serialize_g2(const uint32_t* __restrict__ pts, size_t n, uint8_t* out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  Aff<Fq2> a;
+  load_words(a.x, pts + i * 2 * Fq2::WORDS);
+  load_words(a.y, pts + i * 2 * Fq2::WORDS + Fq2::WORDS);
+  compress_g2(out + SIG_BYTES * i, a.x, a.y);
+}
+
+// ---- host -------------------------------------------------------------------------------------------------------------------------
+struct Timing {
+  float host = 0, hash = 0, kernel = 0;
+};
+inline Timing& last() { static thread_local Timing t; return t; }
+
+using Clock = std::chrono::steady_clock;
+
+// The device side of one batch on the lease's stream: uploads, outputs, and the kernels between events. The destructor zeroes the
+// buffers marked secret on the stream, waits for the stream and frees everything.
+class Batch {
+ public:
+  explicit Batch(cudaStream_t s) : s_(s) {
+    for (auto& e : ev_) B200_CUDA_CHECK(cudaEventCreate(&e));
+  }
+  Batch(const Batch&) = delete;
+  Batch& operator=(const Batch&) = delete;
+  ~Batch() {
+    for (auto& b : bufs_)
+      if (b.secret) cudaMemsetAsync(b.p, 0, b.bytes, s_);
+    cudaStreamSynchronize(s_);
+    for (auto& b : bufs_) cudaFree(b.p);
+    for (auto& e : ev_) cudaEventDestroy(e);
+  }
+  template <class T>
+  const T* in(const T* h, size_t count, bool secret = false) {
+    void* d = alloc(count * sizeof(T), secret);
+    if (count) B200_CUDA_CHECK(cudaMemcpyAsync(d, h, count * sizeof(T), cudaMemcpyHostToDevice, s_));
+    return static_cast<const T*>(d);
+  }
+  uint8_t* out(size_t bytes) { return static_cast<uint8_t*>(alloc(bytes, false)); }
+  // event k before launch k; one more after the last
+  template <class Launch>
+  void run(int k, Launch launch) {
+    B200_CUDA_CHECK(cudaEventRecord(ev_[k], s_));
+    launch(s_);
+    B200_CUDA_CHECK(cudaGetLastError());
+    B200_CUDA_CHECK(cudaEventRecord(ev_[k + 1], s_));
+  }
+  // the milliseconds between events a and b, after the copies back
+  void get(void* h, const void* d, size_t bytes) { B200_CUDA_CHECK(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, s_)); }
+  float ms(int a, int b) {
+    B200_CUDA_CHECK(cudaEventSynchronize(ev_[b]));
+    float t = 0;
+    cudaEventElapsedTime(&t, ev_[a], ev_[b]);
+    return t;
+  }
+
+ private:
+  struct Buf {
+    void* p;
+    size_t bytes;
+    bool secret;
+  };
+  void* alloc(size_t bytes, bool secret) {
+    void* d;
+    B200_CUDA_CHECK(cudaMalloc(&d, bytes + 16));
+    bufs_.push_back({d, bytes + 16, secret});
+    return d;
+  }
+  cudaStream_t s_;
+  cudaEvent_t ev_[3];
+  std::vector<Buf> bufs_;
+};
+
+static unsigned blocks_of(size_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+
+// the call-level checks: n < 2^31, the pointers, and offsets that rise and stay inside the inputs
+static bool calls_ok(size_t n, std::initializer_list<const void*> ptrs, const uint8_t* inputs, size_t inputs_len, const size_t* offsets) {
+  if (n >= LIMIT) return false;
+  if (n == 0) return true;
+  for (const void* p : ptrs)
+    if (!p) return false;
+  if (offsets) {
+    if (!inputs && offsets[n] > offsets[0]) return false;
+    for (size_t i = 0; i < n; i++)
+      if (offsets[i + 1] < offsets[i]) return false;
+    if (offsets[n] > inputs_len) return false;
+  }
+  return true;
+}
+
+static int sign_batch(uint8_t* sigs, uint8_t* statuses, const uint8_t* sks, const uint8_t* inputs, size_t inputs_len,
+                      const size_t* offsets, size_t n) {
+  if (!calls_ok(n, {sigs, statuses, sks, offsets}, inputs, inputs_len, offsets)) return -1;
+  last() = Timing{};
+  if (n == 0) return 0;
+  const auto t0 = Clock::now();
+  std::vector<ethbls::Span> msgs(n);
+  for (size_t i = 0; i < n; i++) msgs[i] = {inputs ? inputs + offsets[i] : nullptr, offsets[i + 1] - offsets[i]};
+  std::vector<uint8_t> uniform;
+  ethbls::expand_all(uniform, msgs.data(), n);
+  Timing t;
+  t.host = (float)ms_since(t0);
+  EngineLease lease = acquire_engine();
+  {
+    Batch b(lease.e->compute());
+    const uint8_t* d_uni = b.in(uniform.data(), uniform.size());
+    const uint8_t* d_sk = b.in(sks, SK_BYTES * n, true);
+    uint32_t* d_h = reinterpret_cast<uint32_t*>(b.out(G2_AFF * n));
+    uint8_t* d_sig = b.out(SIG_BYTES * n);
+    uint8_t* d_st = b.out(n);
+    b.run(0, [&](cudaStream_t s) { bls::k_bls_hash_to_g2<<<blocks_of(n, bls::H2C_THREADS), bls::H2C_THREADS, 0, s>>>(d_uni, n, d_h); });
+    b.run(1, [&](cudaStream_t s) { k_bls_sign<<<blocks_of(n, THREADS), THREADS, 0, s>>>(d_h, d_sk, n, d_sig, d_st); });
+    b.get(sigs, d_sig, SIG_BYTES * n);
+    b.get(statuses, d_st, n);
+    t.hash = b.ms(0, 1);
+    t.kernel = b.ms(1, 2);
+  }
+  last() = t;
+  return 0;
+}
+
+static int derive_batch(uint8_t* pubs, uint8_t* statuses, const uint8_t* sks, size_t n) {
+  if (!calls_ok(n, {pubs, statuses, sks}, nullptr, 0, nullptr)) return -1;
+  last() = Timing{};
+  if (n == 0) return 0;
+  Timing t;
+  EngineLease lease = acquire_engine();
+  {
+    Batch b(lease.e->compute());
+    const uint8_t* d_sk = b.in(sks, SK_BYTES * n, true);
+    uint8_t* d_pub = b.out(PK_BYTES * n);
+    uint8_t* d_st = b.out(n);
+    b.run(0, [&](cudaStream_t s) { k_bls_derive<<<blocks_of(n, THREADS), THREADS, 0, s>>>(d_sk, n, d_pub, d_st); });
+    b.get(pubs, d_pub, PK_BYTES * n);
+    b.get(statuses, d_st, n);
+    t.kernel = b.ms(0, 1);
+  }
+  last() = t;
+  return 0;
+}
+
+static int serialize_batch(bool g2, uint8_t* dst, const void* pts, size_t n) {
+  if (!calls_ok(n, {dst, pts}, nullptr, 0, nullptr)) return -1;
+  last() = Timing{};
+  if (n == 0) return 0;
+  Timing t;
+  EngineLease lease = acquire_engine();
+  {
+    Batch b(lease.e->compute());
+    const uint8_t* d_pts = b.in(static_cast<const uint8_t*>(pts), (g2 ? G2_AFF : G1_AFF) * n);
+    const size_t out_bytes = (g2 ? SIG_BYTES : PK_BYTES) * n;
+    uint8_t* d_out = b.out(out_bytes);
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(d_pts);
+    b.run(0, [&](cudaStream_t s) {
+      if (g2) k_bls_serialize_g2<<<blocks_of(n, 128), 128, 0, s>>>(w, n, d_out);
+      else k_bls_serialize_g1<<<blocks_of(n, 128), 128, 0, s>>>(w, n, d_out);
+    });
+    b.get(dst, d_out, out_bytes);
+    t.kernel = b.ms(0, 1);
+  }
+  last() = t;
+  return 0;
+}
+
+}  // namespace blssign
+}  // namespace b200
+
+using namespace b200;
+
+int ctt_b200_eth_bls_sign_batch(byte* sigs, byte* statuses, const byte* seckeys, const byte* inputs, size_t inputs_len,
+                                const size_t* offsets, size_t n) {
+  return blssign::sign_batch(sigs, statuses, seckeys, inputs, inputs_len, offsets, n);
+}
+
+int ctt_b200_eth_bls_sign(byte sig[96], const byte seckey[32], const byte* msg, size_t msg_len) {
+  if (!msg && msg_len) return -1;
+  static const uint8_t empty = 0;
+  const size_t offsets[2] = {0, msg_len};
+  byte st;
+  if (blssign::sign_batch(sig, &st, seckey, msg ? msg : &empty, msg_len, offsets, 1) != 0) return -1;
+  return st;
+}
+
+int ctt_b200_eth_bls_derive_pubkey_batch(byte* pubkeys, byte* statuses, const byte* seckeys, size_t n) {
+  return blssign::derive_batch(pubkeys, statuses, seckeys, n);
+}
+
+int ctt_b200_eth_bls_derive_pubkey(byte pubkey[48], const byte seckey[32]) {
+  byte st;
+  if (blssign::derive_batch(pubkey, &st, seckey, 1) != 0) return -1;
+  return st;
+}
+
+int ctt_b200_eth_bls_serialize_pubkey_compressed(byte dst[48], const void* pubkey) {
+  if (!dst || !pubkey) return -1;
+  bls12_381::Fp x, y;
+  memcpy(x.l, pubkey, 48);
+  memcpy(y.l, (const uint8_t*)pubkey + 48, 48);
+  bls12_381::compress_g1(dst, x, y, x.is_zero() && y.is_zero());
+  return 0;
+}
+
+int ctt_b200_eth_bls_serialize_signature_compressed(byte dst[96], const void* sig) {
+  if (!dst || !sig) return -1;
+  bls12_381::Fp c[4];   // x.c0, x.c1, y.c0, y.c1
+  for (int k = 0; k < 4; k++) memcpy(c[k].l, (const uint8_t*)sig + 48 * k, 48);
+  const bool inf = c[0].is_zero() && c[1].is_zero() && c[2].is_zero() && c[3].is_zero();
+  bls12_381::compress_g2(dst, c[0], c[1], c[2], c[3], inf);
+  return 0;
+}
+
+int ctt_b200_eth_bls_serialize_pubkeys_compressed_batch(byte* dst, const void* pubkeys, size_t n) {
+  return blssign::serialize_batch(false, dst, pubkeys, n);
+}
+
+int ctt_b200_eth_bls_serialize_signatures_compressed_batch(byte* dst, const void* sigs, size_t n) {
+  return blssign::serialize_batch(true, dst, sigs, n);
+}
+
+void ctt_b200_eth_bls_signer_last_timing(float* ms_host, float* ms_hash, float* ms_kernel) {
+  if (ms_host) *ms_host = blssign::last().host;
+  if (ms_hash) *ms_hash = blssign::last().hash;
+  if (ms_kernel) *ms_kernel = blssign::last().kernel;
+}

@@ -1,5 +1,5 @@
 // BLS12-381 host-side codec pieces shared by the EIP-2537 entries (evm_bls12381_msm.cu) and the EIP-4844 entries
-// (eth_kzg_commit.cu): the group order, the prime-order subgroup check and the 48-byte compressed G1 format.
+// (eth_kzg_commit.cu): the group order, the prime-order subgroup check and the compressed G1 and G2 formats.
 // Host code only (tiny, per-input work next to the GPU MSM); compiles with a plain C++ compiler as well (tests/ builds it with g++).
 #pragma once
 #include <cstdint>
@@ -45,8 +45,8 @@ static Fp fp_pow(const Fp& a, const uint64_t e[6]) {
   return r;
 }
 
-// y > (p - 1) / 2 as integers ("lexicographically largest", the sign bit of the compressed format)
-static bool is_lexicographically_largest(const Fp& y_mont) {
+// -1, 0 or 1 as y is below, equal to or above (p - 1) / 2, as integers
+static int compare_half(const Fp& y_mont) {
   const Fp y = from_mont(y_mont);
   uint64_t half[6];   // (p - 1) / 2
   {
@@ -56,11 +56,14 @@ static bool is_lexicographically_largest(const Fp& y_mont) {
     for (int i = 0; i < 6; i++) half[i] = (t[i] >> 1) | (i + 1 < 6 ? t[i + 1] << 63 : 0);
   }
   for (int i = 5; i >= 0; i--) {
-    if (y.l[i] > half[i]) return true;
-    if (y.l[i] < half[i]) return false;
+    if (y.l[i] > half[i]) return 1;
+    if (y.l[i] < half[i]) return -1;
   }
-  return false;
+  return 0;
 }
+
+// y > (p - 1) / 2 as integers ("lexicographically largest", the sign bit of the compressed format)
+static bool is_lexicographically_largest(const Fp& y_mont) { return compare_half(y_mont) > 0; }
 
 // 48-byte compressed G1 (ZCash flags: 0x80 compressed, 0x40 infinity, 0x20 y is the larger root) -> affine Montgomery (x, y);
 // infinity -> (0, 0). No subgroup check (trusted-setup points; the reference checks them when it loads the file).
@@ -98,17 +101,36 @@ static int decompress_g1(Fp& x, Fp& y, const uint8_t src[48]) {
   return Success;
 }
 
-static void compress_g1(uint8_t dst[48], const Fp& x_mont, const Fp& y_mont, bool inf) {
-  memset(dst, 0, 48);
-  if (inf) { dst[0] = 0xC0; return; }
+// 48 big-endian bytes of x (canonical, from Montgomery form)
+static void store_be48(uint8_t dst[48], const Fp& x_mont) {
   const Fp x = from_mont(x_mont);
   for (int limb = 0; limb < 6; limb++) {
     uint64_t v = x.l[limb];
     uint8_t* p = dst + (5 - limb) * 8;
     for (int b = 7; b >= 0; b--) { p[b] = (uint8_t)v; v >>= 8; }
   }
+}
+
+// The compressed formats as the reference's serialize_g1_compressed / serialize_g2_compressed write them
+// (constantine/serialization/codecs_bls12_381.nim): infinity is 0xC0 then zeros; otherwise 0x80 | 0x20 when y is the larger root.
+// G1 sets 0x20 for y >= (p - 1) / 2. No point of E(Fp) has y = (p - 1) / 2 (((p - 1) / 2)^2 - 4 is not a cube mod p), so on the
+// curve this is the decoder's y > (p - 1) / 2. Neither checks the curve or the subgroup.
+static void compress_g1(uint8_t dst[48], const Fp& x_mont, const Fp& y_mont, bool inf) {
+  memset(dst, 0, 48);
+  if (inf) { dst[0] = 0xC0; return; }
+  store_be48(dst, x_mont);
   dst[0] |= 0x80;
-  if (is_lexicographically_largest(y_mont)) dst[0] |= 0x20;
+  if (compare_half(y_mont) >= 0) dst[0] |= 0x20;
+}
+
+// G2: x.c1 then x.c0; 0x20 when y.c1 > (p - 1) / 2, or y.c0 > (p - 1) / 2 when y.c1 = 0 (the reference compares with (p + 1) / 2)
+static void compress_g2(uint8_t dst[96], const Fp& x0, const Fp& x1, const Fp& y0, const Fp& y1, bool inf) {
+  memset(dst, 0, 96);
+  if (inf) { dst[0] = 0xC0; return; }
+  store_be48(dst, x1);
+  store_be48(dst + 48, x0);
+  dst[0] |= 0x80;
+  if (is_lexicographically_largest(y1.is_zero() ? y0 : y1)) dst[0] |= 0x20;
 }
 
 }  // namespace bls12_381

@@ -1013,6 +1013,96 @@ def eth_bls_last_timing() -> dict:
     return dict(zip(("ms_host", "ms_hash", "ms_blind", "ms_msm", "ms_miller", "ms_final"), (x.value for x in v)))
 
 
+BLS_SCALAR_STATUS = ("cttCodecScalar_Success", "cttCodecScalar_Zero", "cttCodecScalar_ScalarLargerThanCurveOrder")
+
+
+def _bls_sign_call(name, *args):
+    rc = getattr(_lib.load(), "ctt_b200_eth_bls_" + name)(*args)
+    if rc < 0:
+        raise ValueError("ctt_b200_eth_bls_%s: invalid call" % name)
+    return rc
+
+
+def _bls_sign_batch(name, n, out_size, *args):
+    if n == 0:
+        return []
+    st = ctypes.create_string_buffer(n)
+    out = ctypes.create_string_buffer(out_size * n)
+    _bls_sign_call(name + "_batch", out, st, *args)
+    sts, raw = st.raw, out.raw
+    return [(BLS_SCALAR_STATUS[sts[i]], raw[out_size * i:out_size * (i + 1)]) for i in range(n)]
+
+
+def eth_bls_sign(seckey: bytes, msg: bytes):
+    """Ethereum BLS signature of msg (DST BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_POP_) under the 32-byte big-endian secret key,
+    through ctt_b200_eth_bls_sign: (status name, 96-byte compressed signature; zeros unless the status is Success)."""
+    msg = bytes(msg)
+    out = ctypes.create_string_buffer(96)
+    return BLS_SCALAR_STATUS[_bls_sign_call("sign", out, bytes(seckey), msg, len(msg))], out.raw
+
+
+def eth_bls_derive_pubkey(seckey: bytes):
+    """ctt_b200_eth_bls_derive_pubkey: (status name, 48-byte compressed [sk]G1)."""
+    out = ctypes.create_string_buffer(48)
+    return BLS_SCALAR_STATUS[_bls_sign_call("derive_pubkey", out, bytes(seckey))], out.raw
+
+
+def eth_bls_sign_batch(seckeys, msgs) -> list:
+    """n signatures in one pass (ctt_b200_eth_bls_sign_batch): lists of secret keys and messages -> [(status name, 96 bytes)]."""
+    n = len(msgs)
+    return _bls_sign_batch("sign", n, 96, _ecdsa_joined(seckeys, 32, n), *_ecdsa_messages(msgs), n)
+
+
+def eth_bls_derive_pubkey_batch(seckeys) -> list:
+    """n public keys in one pass (ctt_b200_eth_bls_derive_pubkey_batch) -> [(status name, 48 bytes)]."""
+    n = len(seckeys)
+    return _bls_sign_batch("derive_pubkey", n, 48, _ecdsa_joined(seckeys, 32, n), n)
+
+
+def _serialize_batch(name, items, in_size, out_size, what):
+    src, n = _compressed_items(items, in_size, what)
+    if n == 0:
+        return []
+    out = ctypes.create_string_buffer(out_size * n)
+    _bls_sign_call(name, out, _buf(src), n)
+    raw = out.raw
+    return [raw[out_size * i:out_size * (i + 1)] for i in range(n)]
+
+
+def eth_bls_serialize_pubkeys(pubkeys) -> list:
+    """ctt_eth_bls_pubkey structs (96 bytes, a list or one joined buffer) compressed on the GPU
+    (ctt_b200_eth_bls_serialize_pubkeys_compressed_batch) -> [48 bytes]."""
+    return _serialize_batch("serialize_pubkeys_compressed_batch", pubkeys, ETH_BLS_PUBKEY_BYTES, 48, "public key struct")
+
+
+def eth_bls_serialize_signatures(sigs) -> list:
+    """ctt_eth_bls_signature structs (192 bytes) compressed on the GPU (ctt_b200_eth_bls_serialize_signatures_compressed_batch)
+    -> [96 bytes]."""
+    return _serialize_batch("serialize_signatures_compressed_batch", sigs, ETH_BLS_SIGNATURE_BYTES, 96, "signature struct")
+
+
+def eth_bls_serialize_pubkey(pubkey: bytes) -> bytes:
+    """ctt_b200_eth_bls_serialize_pubkey_compressed on the host: a 96-byte struct -> 48 bytes."""
+    out = ctypes.create_string_buffer(48)
+    _bls_sign_call("serialize_pubkey_compressed", out, _buf(_compressed_items([pubkey], ETH_BLS_PUBKEY_BYTES, "public key struct")[0]))
+    return out.raw
+
+
+def eth_bls_serialize_signature(sig: bytes) -> bytes:
+    """ctt_b200_eth_bls_serialize_signature_compressed on the host: a 192-byte struct -> 96 bytes."""
+    out = ctypes.create_string_buffer(96)
+    _bls_sign_call("serialize_signature_compressed", out, _buf(_compressed_items([sig], ETH_BLS_SIGNATURE_BYTES, "signature struct")[0]))
+    return out.raw
+
+
+def eth_bls_signer_last_timing() -> dict:
+    """The calling thread's last BLS signing call (ms): host expand_message_xmd, the hash-to-G2 kernel and the multiplication and
+    compression kernel (CUDA events)."""
+    v = [ctypes.c_float(0) for _ in range(3)]
+    _lib.load().ctt_b200_eth_bls_signer_last_timing(*[ctypes.byref(x) for x in v])
+    return dict(zip(("ms_host", "ms_hash", "ms_kernel"), (x.value for x in v)))
+
+
 class EthKzgContext:
     """EIP-4844 commitment context on the resident SRS, the role of the reference's EthereumKZGContext for
     blob_to_kzg_commitment[_parallel] (reference constantine/ethereum_eip4844_kzg_parallel.nim:125-159)."""

@@ -20,6 +20,11 @@ Nothing here is copied from a table: every constant is computed from the curve.
     the G1 generator. It goes to constantine_b200/csrc/codec_constants.cuh (the decoders of codec_g1.cuh / codec_kernels.cuh).
   - [1..8]G1, affine, the constant table of the joint scalar multiplication (ecops::joint_mul) in the KZG opening check of the
     point-evaluation precompile.
+  - The fixed-base table of the key-derivation kernel (bls_ct.cuh): [j 16^i]G1 for 64 windows i and j = 1..15, built by repeated
+    addition of 16^i G1; every entry is checked on the curve, rows are checked against an independent double-and-add, and no entry
+    is infinity (r is prime and does not divide j 16^i), so the complete addition's (0 : 1 : 0) for a zero digit is the only
+    infinity the kernel selects. It goes to constantine_b200/csrc/bls_ct_table.cuh, which is not kept in git: the library's Makefile
+    runs `gen_bls_constants.py --ct-table` to make it (that mode writes nothing else and skips the isogeny searches).
 """
 import json
 import os
@@ -34,6 +39,8 @@ FIXTURE = os.path.join(ROOT, "tests", "golden", "bls_kat.json")
 FIXTURE_G1 = os.path.join(ROOT, "tests", "golden", "eip2537_pairing_map_kat.json")
 OUT = os.path.join(ROOT, "constantine_b200", "csrc", "bls_constants.cuh")
 OUT_CODEC = os.path.join(ROOT, "constantine_b200", "csrc", "codec_constants.cuh")
+OUT_CT = os.path.join(ROOT, "constantine_b200", "csrc", "bls_ct_table.cuh")
+CT_WINDOWS, CT_ENTRIES = 64, 15   # [j 16^i]G1, i < 64, j = 1..15: one complete addition per 4-bit window of a 256-bit scalar
 G1_GEN = (0x17f1d3a73197d7942695638c4fa9ac0fc3688c4f9774b905a14e3a3f171bac586c55e83ff97a1aeffb3af00adb22c6bb,
           0x08b3f481e3aaa0f1a09e30ed741d8ae4fcf5e095d5d00af600db18cb2c04b3edd03cc744a2888ae40caa232946c5e7e1)
 
@@ -674,6 +681,43 @@ def codec_header_text():
     return "\n".join(body)
 
 
+def ct_table():
+    """rows[i][j - 1] = [j 16^i]G1, checked on the curve and against double-and-add"""
+    rows, base = [], G1_GEN
+    for i in range(CT_WINDOWS):
+        row, acc = [], None
+        for j in range(1, CT_ENTRIES + 1):
+            acc = g1_add(acc, base)
+            assert acc is not None and (j * 16 ** i) % R != 0
+            assert (acc[1] * acc[1] - acc[0] ** 3 - 4) % P == 0
+            row.append(acc)
+        assert row[5] == g1_mul(6 * 16 ** i % R, G1_GEN) and row[-1] == g1_mul(15 * 16 ** i % R, G1_GEN)
+        rows.append(row)
+        base = g1_add(row[-1], base)
+    assert g1_mul(R, G1_GEN) is None
+    return rows
+
+
+def ct_header_text():
+    words = [w for row in ct_table() for (x, y) in row for w in mont_words(x) + mont_words(y)]
+    lines = [
+        "// GENERATED by tools/gen_bls_constants.py --ct-table -- the fixed-base table of the BLS key-derivation kernel, see that file.",
+        "// Entry (i, j), i < %d, j = 1..%d: [j 16^i]G1 affine, x then y as 12 Montgomery little-endian words each, at 24 (%d i + j - 1)."
+        % (CT_WINDOWS, CT_ENTRIES, CT_ENTRIES),
+        "#pragma once",
+        "#include <cstdint>",
+        "",
+        "namespace b200 {",
+        "namespace blsct {",
+        "constexpr int CT_WINDOWS = %d, CT_ENTRIES = %d;" % (CT_WINDOWS, CT_ENTRIES),
+        "static __device__ const uint32_t CT_G1_TABLE[%d] = {" % len(words),
+    ]
+    for k in range(0, len(words), 8):
+        lines.append("    " + ", ".join("0x%08xu" % w for w in words[k:k + 8]) + ",")
+    lines += ["};", "}  // namespace blsct", "}  // namespace b200", ""]
+    return "\n".join(lines)
+
+
 def write_if_changed(path, text):
     old = open(path).read() if os.path.exists(path) else None
     if old != text:
@@ -682,6 +726,9 @@ def write_if_changed(path, text):
 
 
 def main():
+    if "--ct-table" in sys.argv[1:]:
+        write_if_changed(OUT_CT, ct_header_text())
+        return
     write_if_changed(OUT, header_text())
     write_if_changed(OUT_CODEC, codec_header_text())
     print("bls constants: one G2 isogeny of %d candidates and one G1 isogeny of 6 match the RFC vectors" % len(iso_candidates()))
