@@ -237,6 +237,15 @@ def load():
         fn.restype = ci
     lib.ctt_b200_eth_bls_signer_last_timing.argtypes = [ctypes.POINTER(ctypes.c_float)] * 3
     lib.ctt_b200_eth_bls_signer_last_timing.restype = None
+    u32 = ctypes.c_uint32
+    for nm, args in (("derive_master_secret_key", [vp, vp, sz]), ("derive_master_secret_keys_batch", [vp, vp, vp, sz, vp, sz]),
+                     ("derive_child_secret_key", [vp, vp, u32]), ("derive_child_secret_keys_batch", [vp, vp, vp, vp, sz]),
+                     ("derive_path_batch", [vp, vp, vp, vp, sz, vp, sz, vp, vp, sz, sz])):
+        fn = getattr(lib, "ctt_b200_eth_eip2333_" + nm)
+        fn.argtypes = args
+        fn.restype = ci
+    lib.ctt_b200_eth_eip2333_last_stats.argtypes = [ctypes.POINTER(ctypes.c_float)] * 2 + [ctypes.POINTER(ctypes.c_uint64)] * 2
+    lib.ctt_b200_eth_eip2333_last_stats.restype = None
     lib.ctt_b200_fft_domain_new.argtypes = [ci, vp, ci, ctypes.POINTER(ci)]
     lib.ctt_b200_fft_domain_new.restype = vp
     lib.ctt_b200_fft_domain_free.argtypes = [vp]

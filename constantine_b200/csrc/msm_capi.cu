@@ -321,6 +321,7 @@ int ctt_b200_sm_count(void) {
 extern "C++" {
 namespace b200 {
 int run_test_secp256k1_field_op(int field_id, int op, void* r, const void* a, const void* b, size_t count);   // evm_secp256k1.cu
+int run_test_eip2333_reduce(int op, void* r, const void* a, size_t count);                                  // eth_bls_keygen.cu
 }
 }
 
@@ -338,6 +339,7 @@ int ctt_b200_test_field_op(int field_id, int op, void* r, const void* a, const v
     case 9: return run_test_field_op<Bn254SnarksFp, 2>(op, r, a, b, count);
     case 11:
     case 12: return run_test_secp256k1_field_op(field_id, op, r, a, b, count);
+    case 13: return run_test_eip2333_reduce(op, r, a, count);
   }
   return -1;
 }

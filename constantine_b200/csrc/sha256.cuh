@@ -107,5 +107,38 @@ B200_DEV void sha256_any(const uint8_t* msg, uint64_t len, uint32_t* h) {
   }
 }
 
+// sha256_any's loop continued from the state h after `done` bytes (a multiple of 64), over msg[0, len) followed by `zeros` zero
+// bytes, with the padding of all done + len + zeros bytes: the inner hash of an HMAC after its key block, where EIP-2333 appends
+// I2OSP(0, 1) to an IKM of any length (eip2333.cuh). Branches on the lengths only.
+B200_DEV void sha256_from(uint32_t* h, uint64_t done, const uint8_t* msg, uint64_t len, uint64_t zeros) {
+  const uint64_t total = len + zeros, blocks = (total + 9 + 63) / 64, bits = (done + total) * 8;
+#pragma unroll 1
+  for (uint64_t blk = 0; blk < blocks; blk++) {
+    uint32_t w[16];
+    const uint64_t base = 64 * blk;
+    if (base + 64 <= len) {
+#pragma unroll
+      for (int i = 0; i < 16; i++) {
+        const uint8_t* p = msg + base + 4 * i;
+        w[i] = ((uint32_t)__ldg(p) << 24) | ((uint32_t)__ldg(p + 1) << 16) | ((uint32_t)__ldg(p + 2) << 8) | __ldg(p + 3);
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 16; i++) {
+        uint32_t v = 0;
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          const uint64_t at = base + 4 * i + j;
+          const uint32_t byte = at < len ? __ldg(msg + at) : (at == total ? 0x80u : 0u);
+          v = (v << 8) | byte;
+        }
+        w[i] = v;
+      }
+      if (blk + 1 == blocks) { w[14] = (uint32_t)(bits >> 32); w[15] = (uint32_t)bits; }
+    }
+    compress(h, w);
+  }
+}
+
 }  // namespace sha256
 }  // namespace b200

@@ -16,6 +16,7 @@ reference's C structs (see include/ctt_b200_msm.h). Results come back as `bytes`
 Every call goes through the named extern "C" symbol -- this module adds no arithmetic.
 """
 import ctypes
+import operator
 
 from . import _lib
 from .curves import CURVES, CurveParams
@@ -1101,6 +1102,121 @@ def eth_bls_signer_last_timing() -> dict:
     v = [ctypes.c_float(0) for _ in range(3)]
     _lib.load().ctt_b200_eth_bls_signer_last_timing(*[ctypes.byref(x) for x in v])
     return dict(zip(("ms_host", "ms_hash", "ms_kernel"), (x.value for x in v)))
+
+
+EIP2333_SEED_STATUS = ("Success", "SeedTooShort")
+
+
+def eip2334_path(path: str) -> list:
+    """An EIP-2334 path string ("m/12381/3600/0/0/0") -> its child indices ([12381, 3600, 0, 0, 0]); "m" alone is []. Each index is
+    canonical decimal (no sign, no leading zero, no hardening mark) below 2^32; anything else raises ValueError."""
+    parts = path.split("/")
+    if parts[0] != "m":
+        raise ValueError("an EIP-2334 path starts with m: %r" % path)
+    out = []
+    for p in parts[1:]:
+        if not p or not p.isascii() or not p.isdigit() or (len(p) > 1 and p[0] == "0") or int(p) >= 1 << 32:
+            raise ValueError("bad EIP-2334 path component %r in %r" % (p, path))
+        out.append(int(p))
+    return out
+
+
+def _eip2333_call(name, *args):
+    rc = getattr(_lib.load(), "ctt_b200_eth_eip2333_" + name)(*args)
+    if rc < 0:
+        raise ValueError("ctt_b200_eth_eip2333_%s: invalid call" % name)
+    return rc
+
+
+def _eip2333_index(i):
+    """an index as the C entries take it, a uint32_t: ValueError outside [0, 2^32) rather than ctypes' silent wrap-around"""
+    i = operator.index(i)
+    if not 0 <= i < 1 << 32:
+        raise ValueError("index %d is outside [0, 2^32)" % i)
+    return i
+
+
+def _eip2333_indices(indices, n):
+    indices = [_eip2333_index(i) for i in indices]
+    if len(indices) != n:
+        raise ValueError("%d indices expected" % n)
+    return (ctypes.c_uint32 * max(n, 1))(*indices)
+
+
+def eth_eip2333_derive_master_secret_key(ikm: bytes):
+    """EIP-2333 derive_master_SK(IKM) through ctt_b200_eth_eip2333_derive_master_secret_key: (status name of EIP2333_SEED_STATUS,
+    32-byte big-endian key; zeros for an IKM shorter than 32 bytes)."""
+    ikm = bytes(ikm)
+    out = ctypes.create_string_buffer(32)
+    return EIP2333_SEED_STATUS[_eip2333_call("derive_master_secret_key", out, ikm, len(ikm))], out.raw
+
+
+def eth_eip2333_derive_child_secret_key(parent: bytes, index: int):
+    """EIP-2333 derive_child_SK(parent, index) through ctt_b200_eth_eip2333_derive_child_secret_key: (the parent's
+    BLS_SCALAR_STATUS name, 32-byte key; zeros unless Success)."""
+    out = ctypes.create_string_buffer(32)
+    return BLS_SCALAR_STATUS[_eip2333_call("derive_child_secret_key", out, _ecdsa_joined([parent], 32, 1), _eip2333_index(index))], out.raw
+
+
+def eth_eip2333_derive_master_secret_keys_batch(ikms) -> list:
+    """n master keys in one pass (ctt_b200_eth_eip2333_derive_master_secret_keys_batch) -> [(status name, 32 bytes)]."""
+    ikms = list(ikms)
+    n = len(ikms)
+    if n == 0:
+        return []
+    st, out = ctypes.create_string_buffer(n), ctypes.create_string_buffer(32 * n)
+    _eip2333_call("derive_master_secret_keys_batch", out, st, *_ecdsa_messages(ikms), n)
+    raw = out.raw
+    return [(EIP2333_SEED_STATUS[st.raw[i]], raw[32 * i:32 * i + 32]) for i in range(n)]
+
+
+def eth_eip2333_derive_child_secret_keys_batch(parents, indices) -> list:
+    """n child keys in one pass (ctt_b200_eth_eip2333_derive_child_secret_keys_batch): parents (32 bytes each) and their indices
+    -> [(status name, 32 bytes)]."""
+    parents = list(parents)
+    n = len(parents)
+    if n == 0:
+        return []
+    idx = _eip2333_indices(indices, n)
+    st, out = ctypes.create_string_buffer(n), ctypes.create_string_buffer(32 * n)
+    _eip2333_call("derive_child_secret_keys_batch", out, st, _ecdsa_joined(parents, 32, n), idx, n)
+    raw = out.raw
+    return [(BLS_SCALAR_STATUS[st.raw[i]], raw[32 * i:32 * i + 32]) for i in range(n)]
+
+
+def eth_eip2333_derive_path_batch(seeds, seed_of, paths, secret_keys: bool = True, pubkeys: bool = True) -> list:
+    """Keys along EIP-2334 paths in one call (ctt_b200_eth_eip2333_derive_path_batch). seeds: the distinct seeds; seed_of[i]: the index
+    of item i's seed; paths[i]: its child indices (all of one depth) or a path string for eip2334_path. Common prefixes are derived
+    once. -> [(status name of EIP2333_SEED_STATUS, 32-byte key or None, 48-byte compressed public key or None)], with None for an
+    output not asked for; with secret_keys=False no secret key leaves the device."""
+    seed_of = list(seed_of)
+    paths = [eip2334_path(p) if isinstance(p, str) else list(p) for p in paths]
+    n = len(seed_of)
+    if len(paths) != n:
+        raise ValueError("%d paths expected" % n)
+    if n == 0:
+        return []
+    depth = len(paths[0])
+    if any(len(p) != depth for p in paths):
+        raise ValueError("the paths of one call have one depth")
+    data, data_len, offsets = _ecdsa_messages(list(seeds))
+    flat = _eip2333_indices([x for p in paths for x in p], n * depth)
+    st = ctypes.create_string_buffer(n)
+    sk = ctypes.create_string_buffer(32 * n) if secret_keys else None
+    pk = ctypes.create_string_buffer(48 * n) if pubkeys else None
+    _eip2333_call("derive_path_batch", sk, pk, st, data, data_len, offsets, len(seeds), _eip2333_indices(seed_of, n), flat, depth, n)
+    sks, pks = sk.raw if sk else None, pk.raw if pk else None
+    return [(EIP2333_SEED_STATUS[st.raw[i]], sks[32 * i:32 * i + 32] if sks else None, pks[48 * i:48 * i + 48] if pks else None)
+            for i in range(n)]
+
+
+def eth_eip2333_last_stats() -> dict:
+    """The calling thread's last key-derivation call: ms_host (path planning), ms_kernel (CUDA events), and the master and child
+    derivations that ran."""
+    f = [ctypes.c_float(0) for _ in range(2)]
+    c = [ctypes.c_uint64(0) for _ in range(2)]
+    _lib.load().ctt_b200_eth_eip2333_last_stats(*[ctypes.byref(x) for x in f + c])
+    return {"ms_host": f[0].value, "ms_kernel": f[1].value, "masters": c[0].value, "children": c[1].value}
 
 
 class EthKzgContext:
