@@ -87,6 +87,8 @@ def load():
     lib.ctt_b200_device_count.restype = ci
     lib.ctt_b200_test_field_op.argtypes = [ci, ci, vp, vp, vp, sz]
     lib.ctt_b200_test_field_op.restype = ci
+    lib.ctt_b200_test_ct_op.argtypes = [ci, ci, vp, vp, vp, sz]
+    lib.ctt_b200_test_ct_op.restype = ci
     lib.ctt_b200_test_ec_op.argtypes = [ci, ci, vp, vp, vp, sz]
     lib.ctt_b200_test_ec_op.restype = ci
     if hasattr(lib, "ctt_b200_scalar_mul_u64"):

@@ -110,6 +110,61 @@ static __global__ void __launch_bounds__(128) k_bls_serialize_g2(const uint32_t*
   compress_g2(out + SIG_BYTES * i, a.x, a.y);
 }
 
+// ---- the constant-time test hook (ctt_b200_test_ct_op units 3..6), Montgomery words -------------------------------------------
+// unit 3 Fp (12 words): op 8 ct_fp_inv(a); unit 4 Fp2 (24): op 8 ct_fp2_inv(a); unit 5 G1 (X, Y, Z: 36): op 0 ct_g1_add(a, b),
+// op 2 ct_g1_select(a[0], a[1]); unit 6 G2 (72): op 0 ct_g2_add(a, b), op 1 ct_g2_dbl(a), op 2 ct_g2_select(tab, a[0]) over the
+// caller's table tab = b (16 affine G2 points, entry 0 not read)
+template <class T>
+B200_DEV blsct::Proj<T> load_proj(const uint32_t* p) {
+  blsct::Proj<T> v;
+  load_words(v.x, p);
+  load_words(v.y, p + T::WORDS);
+  load_words(v.z, p + 2 * T::WORDS);
+  return v;
+}
+template <class T>
+B200_DEV void store_proj(uint32_t* p, const blsct::Proj<T>& v) {
+  store_words(p, v.x);
+  store_words(p + T::WORDS, v.y);
+  store_words(p + 2 * T::WORDS, v.z);
+}
+
+static __global__ void __launch_bounds__(THREADS) k_test_ct_op(int unit, int op, uint32_t* r, const uint32_t* a, const uint32_t* b,
+                                                               size_t count) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  if (unit == 3) {
+    Fq x;
+    load_words(x, a + Fq::WORDS * i);
+    store_words(r + Fq::WORDS * i, blsct::ct_fp_inv(x));
+  } else if (unit == 4) {
+    Fq2 x;
+    load_words(x, a + Fq2::WORDS * i);
+    store_words(r + Fq2::WORDS * i, blsct::ct_fp2_inv(x));
+  } else if (unit == 5) {
+    const uint32_t* pa = a + 3 * Fq::WORDS * i;
+    blsct::ProjG1 z = op == 0 ? blsct::ct_g1_add(load_proj<Fq>(pa), load_proj<Fq>(b + 3 * Fq::WORDS * i))
+                              : blsct::ct_g1_select((int)pa[0], pa[1]);
+    store_proj(r + 3 * Fq::WORDS * i, z);
+  } else {
+    const uint32_t* pa = a + 3 * Fq2::WORDS * i;
+    blsct::ProjG2 z;
+    if (op == 0) z = blsct::ct_g2_add(load_proj<Fq2>(pa), load_proj<Fq2>(b + 3 * Fq2::WORDS * i));
+    else if (op == 1) z = blsct::ct_g2_dbl(load_proj<Fq2>(pa));
+    else {
+      // a thread-local copy, as k_bls_sign passes: the selection then compiles as it does there (local loads)
+      Aff<Fq2> tab[16];
+#pragma unroll 1
+      for (int j = 1; j < 16; j++) {
+        load_words(tab[j].x, b + 2 * Fq2::WORDS * j);
+        load_words(tab[j].y, b + 2 * Fq2::WORDS * j + Fq2::WORDS);
+      }
+      z = blsct::ct_g2_select(tab, pa[0]);
+    }
+    store_proj(r + 3 * Fq2::WORDS * i, z);
+  }
+}
+
 // ---- host -------------------------------------------------------------------------------------------------------------------------
 struct Timing {
   float host = 0, hash = 0, kernel = 0;
@@ -194,6 +249,36 @@ static int serialize_batch(bool g2, uint8_t* dst, const void* pts, size_t n) {
 }
 
 }  // namespace blssign
+
+int run_test_bls_ct_op(int unit, int op, void* r, const void* a, const void* b, size_t count) {
+  using namespace blssign;
+  const bool known = ((unit == 3 || unit == 4) && op == 8) || (unit == 5 && (op == 0 || op == 2)) ||
+                     (unit == 6 && (op == 0 || op == 1 || op == 2));
+  if (!known) return -1;
+  if (count == 0) return 0;
+  const bool needs_b = op == 0 || (unit == 6 && op == 2);
+  if (!r || !a || (needs_b && !b) || count >= LIMIT) return -1;
+  const size_t words = unit == 3 ? Fq::WORDS : unit == 4 ? Fq2::WORDS : unit == 5 ? 3 * Fq::WORDS : 3 * Fq2::WORDS;
+  if (op == 2)   // the table row and digit: in range, so the hook reads only the tables
+    for (size_t i = 0; i < count; i++) {
+      const uint32_t* rec = static_cast<const uint32_t*>(a) + words * i;
+      if (unit == 5 ? (rec[0] >= (uint32_t)blsct::CT_WINDOWS || rec[1] > (uint32_t)blsct::CT_ENTRIES) : rec[0] > 15u) return -1;
+    }
+  const size_t bytes = 4 * words * count;
+  const size_t b_bytes = unit == 6 && op == 2 ? 16 * G2_AFF : bytes;
+  EngineLease lease = acquire_engine();
+  {
+    Batch bt(lease.e->compute());
+    const uint32_t* d_a = reinterpret_cast<const uint32_t*>(bt.in(static_cast<const uint8_t*>(a), bytes));
+    const uint32_t* d_b = needs_b ? reinterpret_cast<const uint32_t*>(bt.in(static_cast<const uint8_t*>(b), b_bytes)) : d_a;
+    uint32_t* d_r = reinterpret_cast<uint32_t*>(bt.out(bytes));
+    bt.run(0, [&](cudaStream_t s) { k_test_ct_op<<<blocks_of(count, THREADS), THREADS, 0, s>>>(unit, op, d_r, d_a, d_b, count); });
+    bt.get(r, d_r, bytes);
+    bt.ms(0, 1);
+  }
+  return 0;
+}
+
 }  // namespace b200
 
 using namespace b200;

@@ -229,6 +229,45 @@ static __global__ void __launch_bounds__(THREADS) k_ecdsa_derive(const uint8_t* 
   status[i] = cttEthEcdsa_Success;
 }
 
+// ---- the constant-time test hook (ctt_b200_test_ct_op units 0..2) -------------------------------------------------------------
+// FpC or FrC: op 0 a * b, 1 a + b, 2 a - b, 8 ct_fp_inv / ct_fr_inv of a (8 plain little-endian words each)
+template <class F>
+B200_DEV void test_ct_field(int op, uint32_t* r, const uint32_t* a, const uint32_t* b) {
+  k1::Ct<F> x, y, z = k1::Ct<F>::zero();
+#pragma unroll
+  for (int w = 0; w < 8; w++) { x.l[w] = a[w]; y.l[w] = b[w]; }
+  switch (op) {
+    case 0: z = x * y; break;
+    case 1: z = x + y; break;
+    case 2: z = x - y; break;
+    case 8:
+      if constexpr (F::P(0) == Secp256k1Fp::P(0)) z = k1::ct_fp_inv(x); else z = k1::ct_fr_inv(x);
+      break;
+  }
+#pragma unroll
+  for (int w = 0; w < 8; w++) r[w] = z.l[w];
+}
+
+// unit 0 FpC, 1 FrC (records of 8 words); unit 2 points (X, Y, Z of 8 words each): op 0 ct_point_add(a, b), op 2 ct_select(a[0], a[1])
+static __global__ void k_test_ct_op(int unit, int op, uint32_t* r, const uint32_t* a, const uint32_t* b, size_t count) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  if (unit == 0) { test_ct_field<Secp256k1Fp>(op, r + 8 * i, a + 8 * i, b + 8 * i); return; }
+  if (unit == 1) { test_ct_field<Secp256k1Fr>(op, r + 8 * i, a + 8 * i, b + 8 * i); return; }
+  const uint32_t* pa = a + 24 * i;
+  const uint32_t* pb = b + 24 * i;
+  k1::ProjC p, q, z;
+#pragma unroll
+  for (int w = 0; w < 8; w++) {
+    p.x.l[w] = pa[w]; p.y.l[w] = pa[8 + w]; p.z.l[w] = pa[16 + w];
+    q.x.l[w] = pb[w]; q.y.l[w] = pb[8 + w]; q.z.l[w] = pb[16 + w];
+  }
+  z = op == 0 ? k1::ct_point_add(p, q) : k1::ct_select((int)pa[0], pa[1]);
+  uint32_t* pr = r + 24 * i;
+#pragma unroll
+  for (int w = 0; w < 8; w++) { pr[w] = z.x.l[w]; pr[8 + w] = z.y.l[w]; pr[16 + w] = z.z.l[w]; }
+}
+
 // ---- host -------------------------------------------------------------------------------------------------------------------------
 struct Timing {
   float host = 0, kernel = 0;
@@ -446,6 +485,34 @@ struct One {
 const uint8_t One::empty = 0;
 
 }  // namespace ecdsa
+
+int run_test_ecdsa_ct_op(int unit, int op, void* r, const void* a, const void* b, size_t count) {
+  const bool field = unit == 0 || unit == 1;
+  if (!((field && (op == 0 || op == 1 || op == 2 || op == 8)) || (unit == 2 && (op == 0 || op == 2)))) return -1;
+  if (count == 0) return 0;
+  const bool needs_b = field ? op != 8 : op == 0;   // inverses and selections take one operand
+  if (!r || !a || (needs_b && !b) || count >= (size_t(1) << 31)) return -1;
+  const size_t words = field ? 8 : 24;
+  if (unit == 2 && op == 2)   // the table row and digit: in range, so the hook reads only the table
+    for (size_t i = 0; i < count; i++) {
+      const uint32_t* rec = static_cast<const uint32_t*>(a) + words * i;
+      if (rec[0] >= (uint32_t)k1::CT_WINDOWS || rec[1] > (uint32_t)k1::CT_ENTRIES) return -1;
+    }
+  const size_t bytes = 4 * words * count;
+  EngineLease lease = acquire_engine();
+  cudaStream_t s = lease.e->compute();
+  void *da, *db, *dr;
+  B200_CUDA_CHECK(cudaMalloc(&da, bytes)); B200_CUDA_CHECK(cudaMalloc(&db, bytes)); B200_CUDA_CHECK(cudaMalloc(&dr, bytes));
+  B200_CUDA_CHECK(cudaMemcpyAsync(da, a, bytes, cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(db, needs_b ? b : a, bytes, cudaMemcpyHostToDevice, s));
+  ecdsa::k_test_ct_op<<<ecdsa::blocks(count), ecdsa::THREADS, 0, s>>>(unit, op, (uint32_t*)dr, (const uint32_t*)da, (const uint32_t*)db, count);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpyAsync(r, dr, bytes, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  cudaFree(da); cudaFree(db); cudaFree(dr);
+  return 0;
+}
+
 }  // namespace b200
 
 using namespace b200;

@@ -322,6 +322,8 @@ extern "C++" {
 namespace b200 {
 int run_test_secp256k1_field_op(int field_id, int op, void* r, const void* a, const void* b, size_t count);   // evm_secp256k1.cu
 int run_test_eip2333_reduce(int op, void* r, const void* a, size_t count);                                  // eth_bls_keygen.cu
+int run_test_ecdsa_ct_op(int unit, int op, void* r, const void* a, const void* b, size_t count);             // eth_ecdsa.cu
+int run_test_bls_ct_op(int unit, int op, void* r, const void* a, const void* b, size_t count);               // eth_bls_sign.cu
 }
 }
 
@@ -341,6 +343,12 @@ int ctt_b200_test_field_op(int field_id, int op, void* r, const void* a, const v
     case 12: return run_test_secp256k1_field_op(field_id, op, r, a, b, count);
     case 13: return run_test_eip2333_reduce(op, r, a, count);
   }
+  return -1;
+}
+
+int ctt_b200_test_ct_op(int unit, int op, void* r, const void* a, const void* b, size_t count) {
+  if (unit >= 0 && unit <= 2) return run_test_ecdsa_ct_op(unit, op, r, a, b, count);
+  if (unit >= 3 && unit <= 6) return run_test_bls_ct_op(unit, op, r, a, b, count);
   return -1;
 }
 

@@ -79,7 +79,7 @@ def test_prototypes(kat):
     syms = open(os.path.join(ROOT, "include", "exported_symbols.txt")).read().split()
     for s in list(kat["prototypes"]) + ["ctt_b200_eth_bls_deserialize_pubkey_compressed", "ctt_b200_eth_bls_deserialize_signature_compressed",
                                         "ctt_b200_eth_bls_last_timing", "ctt_b200_test_hash_to_g2", "ctt_b200_test_map_to_g2",
-                                        "ctt_b200_test_pairing"]:
+                                        "ctt_b200_test_pairing", "ctt_b200_test_ct_op"]:
         assert s in syms
 
 
